@@ -27,7 +27,8 @@ static thread_local std::string g_create_error;
 
 namespace {
 
-constexpr unsigned SHARD_RESERVED_SMS = 16;   // SMs K1 leaves to NCCL while an exchange runs beside it
+constexpr unsigned SHARD_RESERVED_SMS = 16;
+constexpr uint64_t WIN_DEF_CAP = (uint64_t)16 << 20;   // deferred records per group of the window form of K2   // SMs K1 leaves to NCCL while an exchange runs beside it
 
 unsigned ceil_log2(uint64_t x) { unsigned l = 0; while(l < 64 && ((uint64_t)1 << l) < x) ++l; return l; }
 unsigned bitsize(uint64_t x) { unsigned b = 0; while(x) { ++b; x >>= 1; } return b ? b : 1; }
@@ -65,11 +66,14 @@ std::vector<uint64_t> build_lut(const jfb::gf2_matrix& m, unsigned nbytes) {
 struct Table {
   unsigned lsize = 0, local_lsize = 0, max_reprobe = 0, rbits = 1, fbits = 1, slot_bits = 32, hb = 0;
   uint64_t size = 0, local_size = 0, margin = 0, local_slots = 0, ovf_size = 0;
+  // slots [materialized, local_size) are zero in meaning but not in memory (table_zero, table_materialize)
+  uint64_t materialized = 0;
   jfb::gf2_matrix M, Minv;
   DevBuf slots, lut, inv_lut, ovf_keys, ovf_vals, lut11;
+  DevBuf win_state;              // while materialized < local_size: one state per window (jf_kernels.cuh, WIN_LAZY ...)
   uint64_t prow[8] = {0,0,0,0,0,0,0,0}; unsigned n_prow = 0; bool hash_fast = false;
   std::vector<uint64_t> reprobes;
-  void release() { slots.free(); lut.free(); inv_lut.free(); ovf_keys.free(); ovf_vals.free(); lut11.free(); }
+  void release() { slots.free(); lut.free(); inv_lut.free(); ovf_keys.free(); ovf_vals.free(); lut11.free(); win_state.free(); }
   size_t bytes() const { return (size_t)local_slots * (slot_bits / 8); }
 };
 
@@ -80,7 +84,7 @@ struct PartState {
   DevBuf pool, dir, order, pool_next, cta_chunk, cta_fill, spill_keys, spill_counts, spill_n, hist, start, cursor, unit_cursor;
   uint64_t spill_cap = 0;
   // window form of K2 (jf_window.cuh)
-  DevBuf w_start, w_cursor, w_cnt, w_rec, w_def_pos, w_def_high, w_def_n;
+  DevBuf w_start, w_cursor, w_cnt, w_rec, w_def_pos[2], w_def_high[2], w_def_n;    // (two deferred lists, w_def_n: their two lengths)
   uint64_t w_rec_cap = 0, w_def_cap = 0;
   uint64_t bound_chunks = 0;     // host-side upper bound of the chunks in use in any one arena
   bool pending = false;          // records sit in the pool
@@ -119,7 +123,7 @@ struct jfgpu_engine {
   jfb::glibc_random rng;
   Table tab;
   DevBuf stats, carry[2], fail_keys[2], fail_counts[2];
-  uint64_t fail_cap = 0;
+  uint64_t fail_cap = 0, fail_group = 0;    // failure list entries; records per group of a careful drain
   int carry_cur = 0, fail_cur = 0;
   unsigned long long* h_stats = nullptr;    // pinned mirror
   // staging for host feeds
@@ -224,14 +228,11 @@ int table_setup(jfgpu_engine* e, Table& t, unsigned lsize, const jfb::gf2_matrix
     return fail(e, JFGPU_ERR_NOMEM, buf);
   }
   t.slots.bytes = t.bytes();
-  CUDA_OK(e, cudaMemsetAsync(t.slots.p, 0, t.bytes(), e->cs));
   // counter-carry side table: one entry per slot whose counter field wrapped; sized with the table
   t.ovf_size = (uint64_t)1 << 20;
   while(t.ovf_size < ((uint64_t)1 << 26) && t.ovf_size * 64 < t.local_size) t.ovf_size <<= 1;
   CUDA_OK(e, t.ovf_keys.alloc(t.ovf_size * 8));
   CUDA_OK(e, t.ovf_vals.alloc(t.ovf_size * 8));
-  CUDA_OK(e, cudaMemsetAsync(t.ovf_keys.p, 0, t.ovf_size * 8, e->cs));
-  CUDA_OK(e, cudaMemsetAsync(t.ovf_vals.p, 0, t.ovf_size * 8, e->cs));
   std::vector<uint64_t> l1 = build_lut(t.M, e->nbytes), l2 = build_lut(t.Minv, e->nbytes);
   CUDA_OK(e, t.lut.alloc(l1.size() * 8));
   CUDA_OK(e, t.inv_lut.alloc(l2.size() * 8));
@@ -265,6 +266,38 @@ int table_setup(jfgpu_engine* e, Table& t, unsigned lsize, const jfb::gf2_matrix
     t.hash_fast = true;
   }
   CUDA_OK(e, cudaStreamSynchronize(e->cs));     // the host vectors are about to go out of scope
+  return JFGPU_OK;
+}
+
+// Zero a table (slots and counter-carry side table) on the compute stream.  `lazy`: slots [0, local_size) are zero in
+// meaning only (materialized = 0, every window WIN_LAZY).  The next drain, window form, writes every window without reading
+// it; the overflow margin past local_size, which deferred probes reach, is zeroed in memory as always.
+int table_zero(jfgpu_engine* e, Table& t, bool lazy) {
+  const size_t sb = t.slot_bits / 8, from = lazy ? (size_t)t.local_size * sb : 0;
+  CUDA_OK(e, cudaMemsetAsync((uint8_t*)t.slots.p + from, 0, t.bytes() - from, e->cs));
+  if(lazy) {
+    const size_t n_win = (size_t)(t.local_size >> WIN_LG) * 4;
+    if(!t.win_state.p) CUDA_OK(e, t.win_state.alloc(n_win));
+    CUDA_OK(e, cudaMemsetAsync(t.win_state.p, 0, n_win, e->cs));
+  }
+  CUDA_OK(e, cudaMemsetAsync(t.ovf_keys.p, 0, t.ovf_size * 8, e->cs));
+  CUDA_OK(e, cudaMemsetAsync(t.ovf_vals.p, 0, t.ovf_size * 8, e->cs));
+  t.materialized = lazy ? 0 : t.local_size;
+  return JFGPU_OK;
+}
+
+// Zero in memory the slots of a lazily zeroed table that no drain has written yet.  Every path that reads or updates
+// slots other than the write-only window drain passes here first: part_drain (L2 and rehash forms, spill list),
+// jfgpu_finish (and so lookup, histogram, dump, max_count and set_op), direct insertion by K1, insert_keys_into and
+// jfgpu_shard_unpack (the record exchange therefore drains with loads, as before).  The
+// window drain calls it itself before it returns, also when it stops for a regrow, so collect never sees such a table.
+int table_materialize(jfgpu_engine* e, Table& t, cudaStream_t st) {
+  if(t.materialized >= t.local_size) return JFGPU_OK;
+  const uint64_t w0 = t.materialized >> WIN_LG;       // (a region boundary; the windows K1 put in memory keep their data)
+  win_zero_kernel<<<e->n_sm * 8, 256, 0, st>>>(t.slots.as<uint32_t>(), t.win_state.as<uint32_t>(), nullptr, w0, (uint32_t)((t.local_size >> WIN_LG) - w0));
+  JF_LAUNCHED();
+  CUDA_OK(e, cudaGetLastError());
+  t.materialized = t.local_size;
   return JFGPU_OK;
 }
 
@@ -320,6 +353,7 @@ PartDev part_dev(const jfgpu_engine* e) {
   d.P = ps.P; d.region_bits = ps.region_bits; d.rec_bytes = ps.rec_bytes; d.cap = ps.cap; d.flush_min = ps.flush_min;
   d.chunk_recs = CHUNK_BYTES / std::max(1u, ps.rec_bytes); d.n_chunks = ps.n_chunks; d.stage_bytes = ps.stage_bytes;
   d.margin = ps.margin;
+  d.lazy_win = e->tab.materialized < e->tab.local_size ? e->tab.win_state.as<uint32_t>() : nullptr;
   d.arena_chunks = ps.arena_chunks;
   d.ring_len = ring_len_for(ps.P ? ps.P : 1);
   d.pool = ps.pool.as<uint8_t>(); d.pool_next = ps.pool_next.as<unsigned int>(); d.n_units = d.pool_next + ps.n_arenas; d.dir = ps.dir.as<uint2>();
@@ -416,7 +450,8 @@ void part_release(jfgpu_engine* e) {
   PartState& ps = e->part;
   ps.pool.free(); ps.dir.free(); ps.order.free(); ps.pool_next.free(); ps.cta_chunk.free(); ps.cta_fill.free();
   ps.spill_keys.free(); ps.spill_counts.free(); ps.spill_n.free(); ps.hist.free(); ps.start.free(); ps.cursor.free(); ps.unit_cursor.free();
-  ps.w_start.free(); ps.w_cursor.free(); ps.w_cnt.free(); ps.w_rec.free(); ps.w_def_pos.free(); ps.w_def_high.free(); ps.w_def_n.free();
+  ps.w_start.free(); ps.w_cursor.free(); ps.w_cnt.free(); ps.w_rec.free(); ps.w_def_n.free();
+  for(int i = 0; i < 2; ++i) { ps.w_def_pos[i].free(); ps.w_def_high[i].free(); }
   ps.w_rec_cap = ps.w_def_cap = 0;
   ps.n_chunks = 0; ps.arena_chunks = 0; ps.n_arenas = 0; ps.pending = false;
 }
@@ -459,6 +494,13 @@ static bool window_enabled(jfgpu_engine* e, const PartDev& pd) {
   return e->p.k2_mode == 0 && e->op == 0 && e->tab.slot_bits == 32 && pd.rec_bytes == 4 && pd.region_bits > WIN_LG &&
          pd.region_bits - WIN_LG <= 11 && CHUNK_BYTES == WIN_NTH * 16;
 }
+// Whether a cleared table may stay zero in meaning only until its first drain: that drain takes the window form (plain
+// insertion, no Bloom prefilter) and then writes every slot of [0, local_size), and a deferred probe reaches less than one
+// region past its window.
+static bool lazy_zero_ok(jfgpu_engine* e) {
+  return e->part.P && e->bloom.mode == BLOOM_NONE && window_enabled(e, part_dev(e)) &&
+         tri(e->tab.max_reprobe) < ((uint64_t)1 << e->part.region_bits);
+}
 int read_stats(jfgpu_engine* e);
 static int window_drain(jfgpu_engine* e, cudaStream_t st, const PartDev& pd, unsigned n_units, bool careful, unsigned group_units,
                         unsigned* done, bool* failed) {
@@ -467,13 +509,38 @@ static int window_drain(jfgpu_engine* e, cudaStream_t st, const PartDev& pd, uns
   const uint32_t wpr_lg = pd.region_bits - WIN_LG;
   if(!ps.w_rec.p) {
     ps.w_rec_cap = (uint64_t)64 << 20;                       // records per group (256 MB)
-    ps.w_def_cap = (uint64_t)16 << 20;
+    ps.w_def_cap = WIN_DEF_CAP;
     bool ok = ps.w_rec.alloc(ps.w_rec_cap * 4 + 64) == cudaSuccess && ps.w_start.alloc((((size_t)WIN_MAX_G << 11) + 1) * 4) == cudaSuccess &&
-              ps.w_cursor.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_cnt.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_def_pos.alloc(ps.w_def_cap * 8) == cudaSuccess &&
-              ps.w_def_high.alloc(ps.w_def_cap * 4) == cudaSuccess && ps.w_def_n.alloc(8) == cudaSuccess;
+              ps.w_cursor.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_cnt.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_def_n.alloc(16) == cudaSuccess;
+    for(int i = 0; i < 2 && ok; ++i) ok = ps.w_def_pos[i].alloc(ps.w_def_cap * 8) == cudaSuccess && ps.w_def_high[i].alloc(ps.w_def_cap * 4) == cudaSuccess;
     if(!ok) { cudaGetLastError(); return fail(e, JFGPU_ERR_NOMEM, "device allocation of the window buffers failed"); }
-    CUDA_OK(e, cudaMemsetAsync(ps.w_def_n.p, 0, 8, st));
+    CUDA_OK(e, cudaMemsetAsync(ps.w_def_n.p, 0, 16, st));
   }
+  const TableDev T = table_dev(e, e->tab);
+  // Write-only drain (the table was zeroed lazily; only the windows K1 inserted into are in memory): win_insert2 loads no
+  // other window, win_zero writes the other windows that get no record, and `materialized` follows group by group.  The
+  // deferred records of a group are applied after the next group's windows are written (win_insert2 would overwrite what
+  // they put there), the last group's once the rest of the table is zeroed.  Deferred list of group i: i & 1.
+  bool zero = e->tab.materialized == 0;
+  int def_wait = -1;                                         // deferred list not applied yet
+  auto run_deferred = [&](int set) {
+    WinDev wd;
+    memset(&wd, 0, sizeof(wd));
+    wd.def_pos = ps.w_def_pos[set].as<uint64_t>(); wd.def_high = ps.w_def_high[set].as<uint32_t>();
+    wd.def_n = ps.w_def_n.as<unsigned long long>() + set; wd.def_cap = ps.w_def_cap;
+    if(e->kw == 1) win_deferred_kernel<1><<<e->n_sm * 2, 256, 0, st>>>(T, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
+    else           win_deferred_kernel<2><<<e->n_sm * 2, 256, 0, st>>>(T, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
+    JF_LAUNCHED();
+    cudaMemsetAsync(wd.def_n, 0, 8, st);
+  };
+  auto end_zero = [&]() -> int {                             // the rest of the table in memory, then the waiting deferred records
+    if(!zero) return JFGPU_OK;
+    const int rc = table_materialize(e, e->tab, st);
+    if(rc) return rc;
+    if(def_wait >= 0) run_deferred(def_wait);
+    def_wait = -1; zero = false;
+    return JFGPU_OK;
+  };
   // first unit of every region (chunk_scan_kernel wrote it), on the host
   std::vector<uint32_t> start(pd.P + 1);
   CUDA_OK(e, cudaMemcpyAsync(start.data(), ps.start.p, (size_t)pd.P * 4, cudaMemcpyDeviceToHost, st));
@@ -486,7 +553,7 @@ static int window_drain(jfgpu_engine* e, cudaStream_t st, const PartDev& pd, uns
   cudaFuncSetAttribute(win_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scatter_smem);
   // (the runs of a group start on 16-byte boundaries: up to 3 padding records per window)
   const uint64_t max_units = std::min<uint64_t>((ps.w_rec_cap - ((uint64_t)WIN_MAX_G << 13)) / pd.chunk_recs, careful ? group_units : 0xFFFFFFFFu);
-  uint32_t gi = 0;
+  uint32_t gi = 0, ng = 0;
   while(r0 < pd.P && *done < n_units) {
     WinDev wd;
     memset(&wd, 0, sizeof(wd));
@@ -499,9 +566,11 @@ static int window_drain(jfgpu_engine* e, cudaStream_t st, const PartDev& pd, uns
       stiles += (nu + WIN_ST_UNITS - 1) / WIN_ST_UNITS;
       ++G;
     }
-    TableDev T = table_dev(e, e->tab);
     if(G == 0) {
-      // a single region holds more records than the group buffer (heavily repeated k-mers): L2 kernel for it
+      // a single region holds more records than the group buffer (heavily repeated k-mers): L2 kernel for it, whose probes
+      // read the slots of the next region too
+      int rc = end_zero();
+      if(rc) return rc;
       const unsigned upto = start[r0 + 1];
       cudaMemsetAsync(ps.unit_cursor.p, 0, 8, st);
       if(e->kw == 1) insert_chunks32_kernel<1><<<e->n_sm * 2, 768, 0, st>>>(T, pd, ps.order.as<uint32_t>(), ps.unit_cursor.as<unsigned int>(), *done, upto, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
@@ -513,9 +582,19 @@ static int window_drain(jfgpu_engine* e, cudaStream_t st, const PartDev& pd, uns
       wd.g0 = r0; wd.G = G; wd.wpr_lg = wpr_lg; wd.n_tiles = tiles;
       wd.wstart = ps.w_start.as<uint32_t>(); wd.wcursor = ps.w_cursor.as<uint32_t>(); wd.wcnt = ps.w_cnt.as<uint32_t>();
       wd.wrec = ps.w_rec.as<uint32_t>(); wd.wrec_cap = ps.w_rec_cap;
-      wd.def_pos = ps.w_def_pos.as<uint64_t>(); wd.def_high = ps.w_def_high.as<uint32_t>();
-      wd.def_n = ps.w_def_n.as<unsigned long long>(); wd.def_cap = ps.w_def_cap;
+      const int set = zero ? (int)(ng & 1) : 0;
+      wd.def_pos = ps.w_def_pos[set].as<uint64_t>(); wd.def_high = ps.w_def_high[set].as<uint32_t>();
+      wd.def_n = ps.w_def_n.as<unsigned long long>() + set; wd.def_cap = ps.w_def_cap;
+      wd.lazy_win = zero ? e->tab.win_state.as<uint32_t>() : nullptr;
       const uint32_t hb = e->tab.fbits - e->tab.rbits;
+      // the deferred records, once every slot they can reach holds its value in memory
+      auto settle = [&]() {
+        if(!zero) { if(tiles) run_deferred(set); return; }
+        e->tab.materialized = (uint64_t)(r0 + G) << pd.region_bits;
+        if(def_wait >= 0) run_deferred(def_wait);
+        def_wait = tiles ? set : -1;
+      };
+      ++ng;
       if(tiles) {
         CUDA_OK(e, cudaMemsetAsync(ps.w_cursor.p, 0, ((size_t)G << wpr_lg) * 4, st));
         win_event(e, st);
@@ -527,24 +606,43 @@ static int window_drain(jfgpu_engine* e, cudaStream_t st, const PartDev& pd, uns
         if(e->kw == 1) {
           cudaFuncSetAttribute(win_insert2_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WIN2_SMEM);
           win_insert2_kernel<1><<<e->n_sm, WIN2_NTH, WIN2_SMEM, st>>>(T, pd, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes); JF_LAUNCHED();
-          win_deferred_kernel<1><<<e->n_sm * 2, 256, 0, st>>>(T, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes); JF_LAUNCHED();
         } else {
           cudaFuncSetAttribute(win_insert2_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WIN2_SMEM);
           win_insert2_kernel<2><<<e->n_sm, WIN2_NTH, WIN2_SMEM, st>>>(T, pd, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes); JF_LAUNCHED();
-          win_deferred_kernel<2><<<e->n_sm * 2, 256, 0, st>>>(T, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes); JF_LAUNCHED();
         }
+        if(zero) {
+          win_zero_kernel<<<e->n_sm * 4, 256, 0, st>>>(e->tab.slots.as<uint32_t>(), wd.lazy_win, wd.wcnt, (uint64_t)r0 << wpr_lg, G << wpr_lg);
+          JF_LAUNCHED();
+        }
+        settle();
         win_event(e, st);
-        CUDA_OK(e, cudaMemsetAsync(ps.w_def_n.p, 0, 8, st));
+      } else {
+        if(zero) {
+          win_zero_kernel<<<e->n_sm * 4, 256, 0, st>>>(e->tab.slots.as<uint32_t>(), wd.lazy_win, nullptr, (uint64_t)r0 << wpr_lg, G << wpr_lg);
+          JF_LAUNCHED();
+        }
+        settle();
       }
       *done = start[r0 + G]; r0 += G;
     }
     if(careful) {
       // the failure counter is looked at one group late, so that the device never waits for the host: two groups of
-      // failed keys fit the failure list (group = fail_cap / 2 records)
+      // failed keys fit the failure list (group = fail_group records), and in a write-only drain the one deferred list that
+      // runs a group later still (fail_cap, jfgpu_create)
       watch_post(e, st, (int)(gi & 1));
-      if(gi > 0 && watch_failed(e, (int)((gi - 1) & 1))) { cudaStreamSynchronize(st); *failed = true; return JFGPU_OK; }
+      if(gi > 0 && watch_failed(e, (int)((gi - 1) & 1))) {
+        // (the old table is collected next: all of it in memory, every deferred record applied)
+        int rc = end_zero();
+        if(rc) return rc;
+        cudaStreamSynchronize(st); *failed = true; return JFGPU_OK;
+      }
       ++gi;
     }
+  }
+  if(zero) {
+    int rc = end_zero();
+    if(rc) return rc;
+    if(careful) { watch_post(e, st, (int)(gi & 1)); ++gi; }      // (the last deferred records may have failed)
   }
   if(careful && gi > 0 && watch_failed(e, (int)((gi - 1) & 1))) { cudaStreamSynchronize(st); *failed = true; return JFGPU_OK; }
   CUDA_OK(e, cudaGetLastError());
@@ -577,7 +675,7 @@ int part_drain(jfgpu_engine* e, cudaStream_t st) {
     CUDA_OK(e, cudaStreamSynchronize(st));
     n_units = std::min(n_units, ps.n_chunks);
   }
-  const unsigned group = careful ? (unsigned)std::max<uint64_t>(1, e->fail_cap / 2 / pd.chunk_recs) : 0xFFFFFFFFu;
+  const unsigned group = careful ? (unsigned)std::max<uint64_t>(1, e->fail_group / pd.chunk_recs) : 0xFFFFFFFFu;
   int rc = JFGPU_OK;
   DevBuf old_inv;     // inverse tables of the geometry the records belong to, once the table has been rebuilt
   unsigned done = 0;
@@ -600,6 +698,7 @@ int part_drain(jfgpu_engine* e, cudaStream_t st) {
       }
     }
   }
+  if(!rc) rc = table_materialize(e, e->tab, st);         // (the L2 and rehash forms and the spill list read the slots)
   unsigned gq = 0;
   if(!rc && !(window_enabled(e, pd) && done >= n_units && !rebuilt))
   do {
@@ -720,6 +819,9 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
     if(ps.bound_chunks + need > ps.arena_chunks) return fail(e, JFGPU_ERR_NOMEM, "record pool smaller than one batch");
     ps.bound_chunks += need;
     ps.pending = true;
+  } else if(mode == 0 && !bc_build) {            // K1 inserts into the table itself
+    rc = table_materialize(e, e->tab, stream);
+    if(rc) return rc;
   }
   const bool shard_send = mode == 3;            // K1 writes region records of the GLOBAL table into the send pool (bank = route_cap)
   const uint32_t tile = (part || shard_send ? 1024 : 512) * 32 - HALO;
@@ -871,10 +973,12 @@ int read_stats(jfgpu_engine* e) {
 
 int insert_keys_into(jfgpu_engine* e, Table& t, const uint64_t* keys, const uint64_t* counts, uint64_t n, cudaStream_t stream) {
   if(n == 0) return JFGPU_OK;
+  int rc = table_materialize(e, t, stream);
+  if(rc) return rc;
   TableDev T = table_dev(e, t);
   const size_t smem = (size_t)e->nbytes * 256 * 8;
   const int grid = (int)std::min<uint64_t>((n + 255) / 256, (uint64_t)e->n_sm * 8);
-  int rc = dispatch(e, e->kw, t.slot_bits, [&](auto KW, auto SB) -> int {
+  rc = dispatch(e, e->kw, t.slot_bits, [&](auto KW, auto SB) -> int {
     auto kern = insert_keys_kernel<decltype(KW)::value, decltype(SB)::value>;
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     kern<<<grid, 256, smem, stream>>>(T, t.lut.as<uint64_t>(), e->nbytes, keys, counts, n);
@@ -957,6 +1061,8 @@ int rebuild_table_impl(jfgpu_engine* e, unsigned nl, const jfb::gf2_matrix& M, i
   Table nt;
   int rc = table_setup(e, nt, nl, M, e->tab.max_reprobe);
   if(rc) { nt.release(); return rc == JFGPU_ERR_NOMEM ? fail(e, JFGPU_ERR_FULL, "Hash full (" + e->err + ")") : rc; }
+  rc = table_zero(e, nt, false);
+  if(rc) { nt.release(); return rc; }
   // distinct / reprobes statistics restart for the new table; STAT_INSERTED counts k-mer
   // occurrences and must not change
   unsigned long long inserted_before = 0;
@@ -997,9 +1103,8 @@ int spill_table(jfgpu_engine* e, uint64_t n_failed) {
   const int hrc = e->spill_fn(e->spill_ctx, e);
   e->in_spill = false;
   if(hrc) return fail(e, JFGPU_ERR_SINK, "the spill hook failed (--disk: writing an intermediate file)");
-  CUDA_OK(e, cudaMemsetAsync(e->tab.slots.p, 0, e->tab.bytes(), e->cs));
-  CUDA_OK(e, cudaMemsetAsync(e->tab.ovf_keys.p, 0, e->tab.ovf_size * 8, e->cs));
-  CUDA_OK(e, cudaMemsetAsync(e->tab.ovf_vals.p, 0, e->tab.ovf_size * 8, e->cs));
+  int rc = table_zero(e, e->tab, false);
+  if(rc) return rc;
   unsigned long long* st = e->stats.as<unsigned long long>();
   CUDA_OK(e, cudaMemsetAsync(st + STAT_DISTINCT, 0, 8, e->cs));       // (statistics of the table restart; STAT_INSERTED counts occurrences and goes on)
   CUDA_OK(e, cudaMemsetAsync(st + STAT_REPROBES, 0, 8, e->cs));
@@ -1013,7 +1118,7 @@ int spill_table(jfgpu_engine* e, uint64_t n_failed) {
     CUDA_OK(e, e->fail_counts[e->fail_cur].alloc(e->fail_cap * 8));
   }
   const uint32_t op = e->op; e->op = 0;
-  int rc = insert_keys_into(e, e->tab, e->fail_keys[old_fail].as<uint64_t>(), e->fail_counts[old_fail].as<uint64_t>(), n_failed, e->cs);
+  rc = insert_keys_into(e, e->tab, e->fail_keys[old_fail].as<uint64_t>(), e->fail_counts[old_fail].as<uint64_t>(), n_failed, e->cs);
   e->op = op;
   if(rc) return rc;
   CUDA_OK(e, cudaStreamSynchronize(e->cs));       // (the keys that had found no slot are counted as inserted now, once)
@@ -1216,7 +1321,11 @@ int jfgpu_create(const jfgpu_params* params, jfgpu_handle* out) {
 
   // side structures
   e->batch_bytes = params->max_batch_bytes ? (size_t)((params->max_batch_bytes + 15) & ~(uint64_t)15) : ((size_t)64 << 20);
-  e->fail_cap = 2 * (uint64_t)e->batch_bytes;      // (two groups of failed keys: the failure counter is read one group late)
+  // The failure counter is read one group late: the list holds the failed keys of two groups, and of one deferred list of
+  // a write-only drain (window_drain: a group's deferred records run after the next group; at most WIN_DEF_CAP records and
+  // at most a group).
+  e->fail_group = e->batch_bytes;
+  e->fail_cap = 2 * e->fail_group + std::min<uint64_t>(WIN_DEF_CAP, e->fail_group);
   bool ok = e->stats.alloc(STAT_N * 8) == cudaSuccess && e->carry[0].alloc(sizeof(Carry)) == cudaSuccess &&
             e->carry[1].alloc(sizeof(Carry)) == cudaSuccess &&
             e->fail_keys[0].alloc(e->fail_cap * 8 * e->kw) == cudaSuccess && e->fail_counts[0].alloc(e->fail_cap * 8) == cudaSuccess &&
@@ -1230,6 +1339,8 @@ int jfgpu_create(const jfgpu_params* params, jfgpu_handle* out) {
   // count --bf-size: mer_dna_bloom_filter(bf_fp, bf_size) in front of the table (count_main.cc:317-321); its matrices are
   // drawn when the first unprimed text arrives
   if(params->bf_size) { rc = bloom_setup(e, BLOOM_FILTER, params->bf_size, params->bf_fp); if(rc) return bail(rc); }
+  rc = table_zero(e, e->tab, lazy_zero_ok(e));
+  if(rc) return bail(rc);
   rc = reset_carry(e, e->cs);
   if(rc) return bail(rc);
   *out = e;
@@ -1550,6 +1661,8 @@ int jfgpu_shard_unpack(jfgpu_handle e, const uint64_t* counts, uint32_t self_ban
   if(ps.bound_chunks + need > ps.arena_chunks) return fail(e, JFGPU_ERR_NOMEM, "record pool smaller than one exchange round");
   ps.bound_chunks += need;
   ps.pending = true;
+  rc = table_materialize(e, e->tab, st);      // (restage_kernel inserts the records of a full ring or chunk into the table itself)
+  if(rc) return rc;
   RestageArgs ra;
   memset(&ra, 0, sizeof(ra));
   ra.T = table_dev(e, e->tab);
@@ -1639,11 +1752,7 @@ int jfgpu_clear(jfgpu_handle e) {
   CUDA_OK(e, cudaStreamSynchronize(e->hs));
   CUDA_OK(e, cudaStreamSynchronize(e->cs));
   resolve_kernel_events(e);
-  if(e->tab.slots.p) {
-    CUDA_OK(e, cudaMemsetAsync(e->tab.slots.p, 0, e->tab.bytes(), e->cs));
-    CUDA_OK(e, cudaMemsetAsync(e->tab.ovf_keys.p, 0, e->tab.ovf_size * 8, e->cs));
-    CUDA_OK(e, cudaMemsetAsync(e->tab.ovf_vals.p, 0, e->tab.ovf_size * 8, e->cs));
-  }
+  if(e->tab.slots.p) { int rc = table_zero(e, e->tab, lazy_zero_ok(e)); if(rc) return rc; }
   if(e->bloom.bits.p && e->bloom.mode != BLOOM_CHECK) CUDA_OK(e, cudaMemsetAsync(e->bloom.bits.p, 0, e->bloom.bits.bytes, e->cs));
   CUDA_OK(e, cudaMemsetAsync(e->stats.p, 0, STAT_N * 8, e->cs));
   if(e->part.pool.p) {
@@ -1690,6 +1799,7 @@ int jfgpu_finish(jfgpu_handle e, jfgpu_stats* s) {
   cudaSetDevice(e->device);
   CUDA_OK(e, cudaStreamSynchronize(e->hs));
   int rc = part_drain(e, e->cs);
+  if(!rc) rc = table_materialize(e, e->tab, e->cs);       // (nothing fed since the table was cleared: no drain ran)
   if(rc) return rc;
   CUDA_OK(e, cudaStreamSynchronize(e->cs));
   CUDA_OK(e, cudaGetLastError());

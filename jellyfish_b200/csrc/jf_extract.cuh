@@ -78,7 +78,7 @@ __device__ __forceinline__ void squeeze(uint64_t& c, uint32_t& b, uint32_t del) 
 // directly after the regions; out of line, it is a cold path.
 template<int KW, int SB>
 __device__ __noinline__ void spill_record(const TableDev T, uint64_t* spill_keys, uint64_t* spill_counts, unsigned long long* spill_n, uint64_t spill_cap,
-                                          uint64_t k0, uint64_t k1, uint64_t pos) {
+                                          uint64_t k0, uint64_t k1, uint64_t pos, uint32_t* lazy_win) {
   // (everything by value: taking the address of the kernel's parameter structures would move them to local memory)
   uint64_t key[KW];
   key[0] = k0; if(KW == 2) key[KW - 1] = k1;
@@ -90,6 +90,10 @@ __device__ __noinline__ void spill_record(const TableDev T, uint64_t* spill_keys
     return;
   }
   // the list is full as well: insert right here (statistics straight to the global counters: the caller's stay in registers)
+  if(SB == 32 && lazy_win) {                       // (only tables of 32-bit slots are zeroed lazily)
+    const uint64_t p = pos & T.local_mask;
+    lazy_win_materialize(lazy_win, (uint32_t*)T.slots, T.local_mask + 1, p, p + tri(T.max_reprobe));
+  }
   LocalStats l = { 0, 0, 0, 0, 0 };
   if(table_add<KW, SB>(T, key, pos, 1, l)) {
     atomicAdd(&T.stats[STAT_INSERTED], 1ull);
@@ -576,7 +580,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
               uint64_t key[KW];
               kmer_at(j, key);
               const uint64_t pos = ((uint64_t)p << f_rgb) | (rec >> f_hb);
-              spill_record<KW, SB>(a.T, pd.spill_keys, pd.spill_counts, pd.spill_n, pd.spill_cap, key[0], key[KW - 1], pos);
+              spill_record<KW, SB>(a.T, pd.spill_keys, pd.spill_counts, pd.spill_n, pd.spill_cap, key[0], key[KW - 1], pos, pd.lazy_win);
             }
           };
 #pragma unroll
@@ -658,7 +662,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
               if(pd.rec_bytes == 4) reinterpret_cast<uint32_t*>(dst)[slot] = (uint32_t)rec.lo;
               else if(pd.rec_bytes == 8) reinterpret_cast<uint64_t*>(dst)[slot] = rec.lo;
               else { reinterpret_cast<uint64_t*>(dst)[2 * slot] = rec.lo; reinterpret_cast<uint64_t*>(dst)[2 * slot + 1] = rec.hi; }
-            } else spill_record<KW, SB>(a.T, pd.spill_keys, pd.spill_counts, pd.spill_n, pd.spill_cap, key[0], key[KW - 1], pos);    // this region's chunk filled up within one window (skewed input)
+            } else spill_record<KW, SB>(a.T, pd.spill_keys, pd.spill_counts, pd.spill_n, pd.spill_cap, key[0], key[KW - 1], pos, pd.lazy_win);    // this region's chunk filled up within one window (skewed input)
           }
         }
         }

@@ -317,6 +317,31 @@ constexpr int PMAX        = 2048;          // partitions (table regions) at most
 constexpr int CHUNK_BYTES = 8192;          // granule of the record pool
 constexpr uint32_t NO_CHUNK = 0xFFFFFFFFu;
 
+// ---- windows of the table and the lazily zeroed table --------------------------------------------
+constexpr uint32_t WIN_LG = 14;                    // slots per window (the unit of K2's window form, jf_window.cuh)
+constexpr uint32_t WIN_SLOTS = 1u << WIN_LG;
+// A table zeroed lazily (jf_engine.cu, table_zero: zero in meaning, garbage in memory until the first drain writes it) keeps one
+// state per window.  A kernel that has to insert into it before that drain -- K1 when the spill list is full -- first puts
+// every window the probe sequence can reach in memory; the drain then loads those windows instead of overwriting them, and
+// table_materialize leaves them alone.
+enum : uint32_t { WIN_LAZY = 0, WIN_ZEROING = 1, WIN_IN_MEMORY = 2 };
+__device__ __noinline__ void lazy_win_materialize(uint32_t* state, uint32_t* tab, uint64_t local_size, uint64_t first_slot, uint64_t last_slot) {
+  const uint64_t w_end = min(last_slot, local_size - 1) >> WIN_LG;          // (the margin past local_size is always in memory)
+  for(uint64_t w = first_slot >> WIN_LG; w <= w_end; ++w) {
+    volatile uint32_t* s = state + w;
+    if(*s == WIN_IN_MEMORY) continue;
+    if(atomicCAS(&state[w], WIN_LAZY, WIN_ZEROING) == WIN_LAZY) {
+      uint4* p = reinterpret_cast<uint4*>(tab + (w << WIN_LG));
+      for(uint32_t i = 0; i < WIN_SLOTS / 4; ++i) p[i] = make_uint4(0, 0, 0, 0);
+      __threadfence();
+      atomicExch(&state[w], WIN_IN_MEMORY);
+    } else {
+      while(*s != WIN_IN_MEMORY) __nanosleep(64);   // another thread is zeroing it
+    }
+  }
+  __threadfence();
+}
+
 struct PartDev {
   uint32_t  P;              // number of regions (power of two)
   uint32_t  region_bits;    // log2(slots per region)
@@ -333,6 +358,8 @@ struct PartDev {
                             // are shared out among the regions, so tables with few regions get long rings
   uint32_t  by_owner;       // sharded counting, send side: regions are those of the GLOBAL table and the arenas belong to the owning
   uint32_t  owner_shift;    // shards (arena = region >> owner_shift), so that a shard's chunks are contiguous for the exchange
+  uint32_t* lazy_win;       // the window states of a table zeroed lazily (jf_engine.cu, table_zero), else null: a direct insertion
+                            // puts the windows it may reach in memory first (lazy_win_materialize)
   uint8_t*  pool;
   unsigned int* pool_next;  // allocation cursor of every arena
   unsigned int* n_units;    // chunks listed in `order` (written by chunk_scan_kernel)

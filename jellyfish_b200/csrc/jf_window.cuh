@@ -14,6 +14,13 @@
 //   win_deferred  the deferred records, with the ordinary global probe sequence, after win_insert
 //        of the same group has completed (stream order), so no slot is ever touched by a window CTA
 //        and by the global path at the same time.
+// The first drain after the table was cleared is WRITE-ONLY (WinDev::lazy_win): the table's slots were not zeroed in memory
+// (jf_engine.cu, table_zero), so win_insert2 zeroes each stage in shared memory instead of loading the window, and
+// win_zero writes the windows that receive no record.  The table then crosses HBM once per drain instead of three times
+// (memset, load, store).  The few windows K1 put in memory for a direct insertion (lazy_win_materialize) are loaded and
+// kept as usual.  A deferred probe of a group's last window may reach into the next group's first window, which
+// that group's win_insert2 writes without reading: the engine applies a group's deferred records after the NEXT group's
+// win_insert2 (two deferred lists).
 // Slots only ever fill up, so a key that left its window because every slot of its sequence inside
 // the window belongs to other keys finds the same situation on every later visit: all its
 // occurrences are deferred, and it cannot end up in two slots.
@@ -21,8 +28,6 @@
 
 namespace jfk {
 
-constexpr uint32_t WIN_LG = 14;                    // slots per window
-constexpr uint32_t WIN_SLOTS = 1u << WIN_LG;
 constexpr uint32_t WIN_TILE_UNITS = 4;             // chunks per partition tile: 8192 records
 constexpr uint32_t WIN_MAX_G = 64;                 // regions per group
 constexpr uint32_t WIN_MAX_WPR = 2048;             // windows per region (region_bits - WIN_LG <= 11)
@@ -30,6 +35,7 @@ constexpr uint32_t WIN_NTH = 512;
 
 struct WinDev {
   uint32_t g0, G, wpr_lg, n_tiles;
+  const uint32_t* lazy_win;                        // write-only drain: the table's window states (only WIN_IN_MEMORY windows are loaded); else null
   uint32_t tile_first[WIN_MAX_G + 1];              // prefix sum of tiles per region of the group (win_hist: WIN_TILE_UNITS chunks)
   uint32_t stile_first[WIN_MAX_G + 1];             // the same for win_scatter's larger tiles (WIN_ST_UNITS chunks)
   uint32_t unit_first[WIN_MAX_G + 1];              // first unit (index into `order`) of each region; [G] = end
@@ -44,6 +50,11 @@ __device__ __forceinline__ uint32_t win_region_of_tile(const WinDev& wd, uint32_
   uint32_t r = 0;
   while(r + 1 < wd.G && wd.tile_first[r + 1] <= tile) ++r;
   return r;
+}
+
+// first slot of window `task` (= region of the group << wpr_lg | window of the region)
+__device__ __forceinline__ uint64_t win_slot_base(const WinDev& wd, uint32_t region_bits, uint32_t task) {
+  return ((uint64_t)(wd.g0 + (task >> wd.wpr_lg)) << region_bits) + ((uint64_t)(task & ((1u << wd.wpr_lg) - 1)) << WIN_LG);
 }
 
 // ---- counts per (region, window) ---------------------------------------------------------------
@@ -213,9 +224,7 @@ __global__ void __launch_bounds__(WIN2_NTH, 1) win_insert2_kernel(TableDev T, Pa
   const uint32_t n_tasks = wd.G << wd.wpr_lg;
   const uint32_t tid = threadIdx.x, lane = tid & 31u;
 
-  auto slot_base_of = [&](uint32_t task) -> uint64_t {
-    return ((uint64_t)(wd.g0 + (task >> wd.wpr_lg)) << pd.region_bits) + ((uint64_t)(task & ((1u << wd.wpr_lg) - 1)) << WIN_LG);
-  };
+  auto slot_base_of = [&](uint32_t task) -> uint64_t { return win_slot_base(wd, pd.region_bits, task); };
   if(tid == 0) {
     mbar_init(&full[0], 1); mbar_init(&full[1], 1);
     mbar_init(&empty[0], WIN2_CONS / 32); mbar_init(&empty[1], WIN2_CONS / 32);     // one arrival per consumer warp
@@ -225,42 +234,59 @@ __global__ void __launch_bounds__(WIN2_NTH, 1) win_insert2_kernel(TableDev T, Pa
 
   if(tid < 32) {
     // ================================= producer =================================
-    if(lane == 0) {
-      uint32_t next_from = blockIdx.x;
-      uint32_t ephase[2] = { 0, 0 };
-      uint32_t cur_task[2] = { WIN2_NONE, WIN2_NONE }, cur_n[2] = { 0, 0 }, cur_b[2] = { 0, 0 };
-      auto load_batch = [&](uint32_t s, uint32_t off, bool with_window) {
-        const uint32_t nb = min(WIN2_RB, cur_n[s] - off);
-        const uint32_t rbytes = ((nb + 3u) & ~3u) * 4u;
-        cursor[s] = 0;
-        mbar_expect_tx(&full[s], rbytes + (with_window ? WIN_SLOTS * 4u : 0u));
-        if(with_window) tma_load_1d(winb0 + s * WIN_SLOTS, tab + slot_base_of(cur_task[s]), WIN_SLOTS * 4u, &full[s]);
-        tma_load_1d(recb0 + s * WIN2_RB, wd.wrec + cur_b[s] + off, rbytes, &full[s]);
-      };
-      auto next_window = [&](uint32_t s) {           // the next non-empty window of this CTA's stride into stage s
-        uint32_t t = next_from, c = 0;
-        while(t < n_tasks && (c = wd.wcnt[t]) == 0) t += gridDim.x;
-        if(t >= n_tasks) { next_from = t; cur_task[s] = WIN2_NONE; info[s].task = WIN2_NONE; mbar_arrive(&full[s]); return; }
-        next_from = t + gridDim.x;
-        cur_task[s] = t; cur_n[s] = c; cur_b[s] = wd.wstart[t];
+    // Lane 0 drives the TMA engine and the barriers; every lane follows the same (uniform) control flow, so that in a
+    // write-only drain the whole warp can zero a stage in place of loading the window.
+    const bool lead = lane == 0;
+    uint32_t next_from = blockIdx.x;
+    uint32_t ephase[2] = { 0, 0 };
+    uint32_t cur_task[2] = { WIN2_NONE, WIN2_NONE }, cur_n[2] = { 0, 0 }, cur_b[2] = { 0, 0 };
+    auto load_batch = [&](uint32_t s, uint32_t off, bool with_window) {     // (lead)
+      const uint32_t nb = min(WIN2_RB, cur_n[s] - off);
+      const uint32_t rbytes = ((nb + 3u) & ~3u) * 4u;
+      cursor[s] = 0;
+      mbar_expect_tx(&full[s], rbytes + (with_window ? WIN_SLOTS * 4u : 0u));
+      if(with_window) tma_load_1d(winb0 + s * WIN_SLOTS, tab + slot_base_of(cur_task[s]), WIN_SLOTS * 4u, &full[s]);
+      tma_load_1d(recb0 + s * WIN2_RB, wd.wrec + cur_b[s] + off, rbytes, &full[s]);
+    };
+    auto next_window = [&](uint32_t s) {             // the next non-empty window of this CTA's stride into stage s
+      uint32_t t = next_from, c = 0;
+      while(t < n_tasks && (c = wd.wcnt[t]) == 0) t += gridDim.x;
+      if(t >= n_tasks) {
+        next_from = t; cur_task[s] = WIN2_NONE;
+        if(lead) { info[s].task = WIN2_NONE; mbar_arrive(&full[s]); }
+        return;
+      }
+      next_from = t + gridDim.x;
+      cur_task[s] = t; cur_n[s] = c; cur_b[s] = wd.wstart[t];
+      const bool fill = wd.lazy_win && wd.lazy_win[slot_base_of(t) >> WIN_LG] != WIN_IN_MEMORY;
+      if(fill) {
+        uint4* const w = reinterpret_cast<uint4*>(winb0 + s * WIN_SLOTS);
+        for(uint32_t i = lane; i < WIN_SLOTS / 4; i += 32) w[i] = make_uint4(0, 0, 0, 0);
+        fence_proxy_async();                         // these writes, before the TMA engine stores the stage
+        __syncwarp();
+      }
+      if(lead) {
         info[s].task = t; info[s].b = cur_b[s]; info[s].n = c;
-        load_batch(s, 0, true);
-      };
-      next_window(0); next_window(1);
-      for(uint32_t s = 0; cur_task[s] != WIN2_NONE; s ^= 1u) {
-        // the consumers work through the batches of stage s in order
-        for(uint32_t off = WIN2_RB; off < cur_n[s]; off += WIN2_RB) {
-          mbar_wait(&empty[s], ephase[s]); ephase[s] ^= 1u;
-          load_batch(s, off, false);
-        }
-        mbar_wait(&empty[s], ephase[s]); ephase[s] ^= 1u;   // every consumer warp is done with this window
+        load_batch(s, 0, !fill);
+      }
+    };
+    next_window(0); next_window(1);
+    for(uint32_t s = 0; cur_task[s] != WIN2_NONE; s ^= 1u) {
+      // the consumers work through the batches of stage s in order
+      for(uint32_t off = WIN2_RB; off < cur_n[s]; off += WIN2_RB) {
+        mbar_wait(&empty[s], ephase[s]); ephase[s] ^= 1u;
+        if(lead) load_batch(s, off, false);
+      }
+      mbar_wait(&empty[s], ephase[s]); ephase[s] ^= 1u;   // every consumer warp is done with this window
+      if(lead) {
         tma_store_1d(tab + slot_base_of(cur_task[s]), winb0 + s * WIN_SLOTS, WIN_SLOTS * 4u);
         tma_commit_group();
         tma_wait_group_read0();                    // the stage may be overwritten
-        next_window(s);
       }
-      tma_wait_group0();                           // every window is back in the table before the kernel ends
+      __syncwarp();
+      next_window(s);
     }
+    if(lead) tma_wait_group0();                    // every window is back in the table before the kernel ends
     return;
   }
 
@@ -348,6 +374,19 @@ __global__ void __launch_bounds__(WIN2_NTH, 1) win_insert2_kernel(TableDev T, Pa
     if(v[0]) atomicAdd(&T.stats[STAT_INSERTED], v[0]);
     if(v[1]) atomicAdd(&T.stats[STAT_DISTINCT], v[1]);
     if(v[2]) atomicAdd(&T.stats[STAT_REPROBES], v[2]);
+  }
+}
+
+// ---- lazily zeroed table: windows [w_first, w_first + n) that are not in memory yet are written as zeros, except those that
+// receive records (wcnt[i] != 0, win_insert2 writes them; wcnt null: none does) -------------------------------------------
+__global__ void __launch_bounds__(256) win_zero_kernel(uint32_t* __restrict__ tab, const uint32_t* __restrict__ state, const uint32_t* __restrict__ wcnt,
+                                                       uint64_t w_first, uint32_t n) {
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t n_warps = gridDim.x * (blockDim.x / 32);
+  for(uint32_t t = (blockIdx.x * blockDim.x + threadIdx.x) / 32; t < n; t += n_warps) {
+    if((wcnt && wcnt[t]) || state[w_first + t] == WIN_IN_MEMORY) continue;
+    uint4* const w = reinterpret_cast<uint4*>(tab + ((w_first + t) << WIN_LG));
+    for(uint32_t i = lane; i < WIN_SLOTS / 4; i += 32) w[i] = make_uint4(0, 0, 0, 0);
   }
 }
 
