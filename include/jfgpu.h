@@ -231,6 +231,23 @@ int  jfgpu_dump(jfgpu_handle h, uint64_t lower, uint64_t upper, uint32_t out_cou
  *    (0 when absent).  Keys not owned by this shard give 0. */
 int  jfgpu_lookup(jfgpu_handle h, const uint64_t* keys, size_t n, uint64_t* vals);
 
+/* -- a database back into a table: binary_query's database (binary_dumper.hpp:148-189) made resident.  `records` (HOST
+ *    memory) holds whole records of a binary/sorted body, ceil(2k/8) little-endian key bytes then counter_len count bytes;
+ *    any number of calls, each record's count is added.  The caller creates the engine with k = key_len/2 and `canonical`
+ *    from the file's header, at least twice as many slots as records and allow_regrow = 1; the engine draws its own hash
+ *    matrix (the database's matrix and size do not matter for look-ups).  The bytes go to the device through a pinned
+ *    staging buffer in slices of at most 64 MB; a doubling during the load keeps the counts.  JFGPU_ERR_ARG: nbytes is
+ *    not a whole number of records or counter_len is outside 1..8; JFGPU_ERR_NOMEM: the database does not fit. */
+int jfgpu_load_records(jfgpu_handle h, const void* records, size_t nbytes, uint32_t counter_len);
+
+/* -- query_from_sequence (sub_commands/query_main.cc:45-51): every k-mer of the text, in input order, as the line
+ *    "MER COUNT\n" (MER in upper case, canonical when the engine is; COUNT 0 when absent).  Same text contract as jfgpu_feed
+ *    (host memory, FILE_BEGIN / FILE_END, FASTA or 4-line FASTQ sniffed per file, no k-mer spans files; -Q does not
+ *    apply).  `sink` is called on the calling thread with consecutive byte ranges of whole lines, in order; a non-zero
+ *    return aborts the query (JFGPU_ERR_SINK).  *n_kmers (may be NULL) = lines written.  The table is not modified. */
+int jfgpu_query(jfgpu_handle h, const char* bytes, size_t n, uint32_t flags,
+                jfgpu_sink_fn sink, void* ctx, uint64_t* n_kmers);
+
 /* -- histogram straight from the resident table (what `jellyfish histo` computes from
  *    the dump, sub_commands/histo_main.cc:33-45): hist[min(count,n_bins-1)]++ for every
  *    distinct k-mer of this shard.  hist: n_bins uint64 in HOST memory. */
@@ -266,6 +283,8 @@ void  jfgpu_host_free(void* p);
 /* cudaMemcpyAsync host->device on `stream` (NULL = legacy default stream) for callers that have no
  * CUDA binding of their own; with memory from jfgpu_host_alloc the copy is asynchronous. */
 int   jfgpu_memcpy_h2d(void* dev_dst, const void* host_src, size_t bytes, void* stream);
+/* Number of CUDA devices visible to this process (0 without a device or a driver): lets a caller pick a CPU path. */
+int   jfgpu_device_count(void);
 /* Number of engine kernels launched so far by this process (bench "gpu_launches"). */
 uint64_t jfgpu_kernel_launches(void);
 const char* jfgpu_version(void);

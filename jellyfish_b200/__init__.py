@@ -7,6 +7,6 @@ Package contents (only what the path needs):
   engine.py       Python mirror of the reference's hash_counter / dumper interfaces
   distributed.py  one-process-per-GPU sharded counting over torch.distributed
 """
-from .engine import HashCounter, BloomCounter, ReadMerFile, JellyfishError, reference_matrix, mer_to_int, int_to_mer, canonical_int  # noqa: F401
+from .engine import HashCounter, BloomCounter, ReadMerFile, JellyfishError, reference_matrix, mer_to_int, int_to_mer, canonical_int, load_database  # noqa: F401
 
-__all__ = ["HashCounter", "BloomCounter", "ReadMerFile", "JellyfishError", "reference_matrix", "mer_to_int", "int_to_mer", "canonical_int"]
+__all__ = ["HashCounter", "BloomCounter", "ReadMerFile", "JellyfishError", "reference_matrix", "mer_to_int", "int_to_mer", "canonical_int", "load_database"]

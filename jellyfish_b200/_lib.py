@@ -19,6 +19,7 @@ SYMBOLS = [
     "jfgpu_host_alloc", "jfgpu_host_free", "jfgpu_memcpy_h2d", "jfgpu_kernel_launches", "jfgpu_version",
     "jfgpu_bloom_info_get", "jfgpu_bloom_load", "jfgpu_bloom_dump",
     "jfgpu_set_spill", "jfgpu_shard_setup", "jfgpu_shard_round_bytes", "jfgpu_shard_extract", "jfgpu_shard_pack", "jfgpu_shard_unpack",
+    "jfgpu_load_records", "jfgpu_query", "jfgpu_device_count",
 ]
 
 OK, ERR_ARG, ERR_CUDA, ERR_FULL, ERR_FORMAT, ERR_STATE, ERR_NOMEM, ERR_SINK = range(8)
@@ -150,5 +151,11 @@ def load():
     lib.jfgpu_shard_pack.restype = C.c_int
     lib.jfgpu_shard_unpack.argtypes = [H, C.POINTER(C.c_uint64), C.c_uint32, C.c_void_p]
     lib.jfgpu_shard_unpack.restype = C.c_int
+    lib.jfgpu_load_records.argtypes = [H, C.c_void_p, C.c_size_t, C.c_uint32]
+    lib.jfgpu_load_records.restype = C.c_int
+    lib.jfgpu_query.argtypes = [H, C.c_void_p, C.c_size_t, C.c_uint32, SINK_FN, C.c_void_p, C.POINTER(C.c_uint64)]
+    lib.jfgpu_query.restype = C.c_int
+    lib.jfgpu_device_count.argtypes = []
+    lib.jfgpu_device_count.restype = C.c_int
     _lib = lib
     return lib

@@ -3,7 +3,7 @@
 //
 //   jellyfish-b200 count  ...   switches of sub_commands/count_main_cmdline.yaggo:4-112
 //   jellyfish-b200 dump   ...   sub_commands/dump_main_cmdline.yaggo  (CPU reader of the format)
-//   jellyfish-b200 query  ...   sub_commands/query_main_cmdline.yaggo (CPU reader of the format)
+//   jellyfish-b200 query  ...   sub_commands/query_main_cmdline.yaggo (-s on the GPU when there is one, else a CPU reader)
 //   jellyfish-b200 info / histo / stats / merge      small CPU readers used by the tests
 //
 // The flow of `count` mirrors count_main (sub_commands/count_main.cc:218-385): header
@@ -576,6 +576,37 @@ uint64_t db_lookup(const db_reader& db, const uint64_t* key) {
   return 0;
 }
 
+// query -s on the device (query_from_sequence, query_main.cc:45-51): the database's records go into a table of this GPU (its own
+// hash matrix, twice as many slots as records), then every -s file streams through jfgpu_query into `out`
+void query_sequences_device(const db_reader& db, const std::vector<const char*>& sequences, FILE* out) {
+  jfgpu_params p;
+  memset(&p, 0, sizeof(p));
+  p.struct_size = sizeof(p);
+  p.k = db.k; p.size = std::max<uint64_t>(2 * (uint64_t)db.n_records, 2); p.counter_len = 7; p.max_reprobe = 126;
+  p.canonical = db.header.canonical(); p.allow_regrow = 1; p.n_shards = 1;
+  jfgpu_handle h = nullptr;
+  if(jfgpu_create(&p, &h) != JFGPU_OK) die(std::string("Failed to create the device hash: ") + jfgpu_last_error(nullptr));
+  const size_t slice = std::max<size_t>(((size_t)1 << 30) / db.rec, 1) * db.rec;      // whole records of the mapped body
+  const size_t body = db.n_records * db.rec;
+  for(size_t off = 0; off < body; off += slice)
+    if(jfgpu_load_records(h, db.base + db.body_off + off, std::min(slice, body - off), db.counter_len) != JFGPU_OK)
+      die(std::string("Failed to load the database into the device hash: ") + jfgpu_last_error(h));
+  bool write_ok = true;                         // (the engine hands over up to 64 MB of lines at a time: large fwrites)
+  auto sink = [](void* ctx, const void* lines, size_t n) -> int {
+    std::pair<FILE*, bool*>* c = (std::pair<FILE*, bool*>*)ctx;
+    if(fwrite(lines, 1, n, c->first) != n) { *c->second = false; return 1; }
+    return 0;
+  };
+  std::pair<FILE*, bool*> sc(out, &write_ok);
+  jfb::input_buffers mem = { [](size_t n) { return jfgpu_host_alloc(n); }, [](void* q) { jfgpu_host_free(q); } };
+  const std::string err = jfb::stream_inputs(sequences, jfb::generator_spec(), mem,
+    [&](const char* data, size_t n, uint32_t flags) { return jfgpu_query(h, data, n, flags, sink, &sc, nullptr); },
+    [&]() { return std::string(write_ok ? jfgpu_last_error(h) : "Error writing the query output"); });
+  if(!err.empty()) die(err);
+  if(fflush(out) != 0) die("Error writing the query output");
+  jfgpu_destroy(h);
+}
+
 int query_main(int argc, char* argv[]) {
   std::vector<const char*> sequences; const char* output = nullptr; bool interactive = false;
   static struct option longs[] = { {"sequence", required_argument, 0, 's'}, {"output", required_argument, 0, 'o'},
@@ -599,7 +630,10 @@ int query_main(int argc, char* argv[]) {
     if(canonical) { reverse_complement(m, db.k, r); if(mer_less(r, m)) q = r; }
     fprintf(out, "%s %llu\n", mer_to_string(q, db.k).c_str(), (unsigned long long)db_lookup(db, q));
   };
-  for(const char* path : sequences) {          // every k-mer of the sequence files, in order
+  // every k-mer of the sequence files, in order: on the GPU when there is one, else with the binary search below
+  const bool on_device = !sequences.empty() && jfgpu_device_count() > 0;
+  if(on_device) query_sequences_device(db, sequences, out);
+  if(!on_device) for(const char* path : sequences) {
     std::ifstream is(path);
     if(!is.good()) die(std::string("Can't open file '") + path + "'");
     std::string line, seq;

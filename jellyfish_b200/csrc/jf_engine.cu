@@ -17,6 +17,7 @@
 #include "jf_window.cuh"
 #include "jf_dump.cuh"
 #include "jf_shard.cuh"
+#include "jf_query.cuh"
 
 using namespace jfk;
 
@@ -158,6 +159,17 @@ struct jfgpu_engine {
   double win_ms[3] = { 0, 0, 0 };
   // failure counter watched one group behind (hash_counter::add -> handle_full_ary), without draining the stream
   unsigned long long* h_watch = nullptr; cudaEvent_t ev_watch[2] = { nullptr, nullptr };
+  // jfgpu_query: two sets of per-batch buffers (the lines of batch i are copied out while batch i+1 is looked up)
+  bool querying = false;
+  struct QueryBufs {
+    DevBuf keys, vals, cnt, off, out;
+    unsigned long long* h_off = nullptr;    // pinned copy of `off` (entry n_tiles: the batch's total)
+    uint32_t* h_cnt = nullptr;              // pinned copy of `cnt`
+    uint64_t n_tiles = 0;
+    cudaEvent_t ev_front = nullptr, ev_fmt = nullptr;
+  } qb[2];
+  uint8_t* q_host[2] = { nullptr, nullptr }; cudaEvent_t ev_qcopy[2] = { nullptr, nullptr };
+  uint64_t q_tiles_cap = 0; int q_cur = 0;
 };
 
 namespace {
@@ -790,9 +802,11 @@ size_t part_cap_len(const jfgpu_engine* e, size_t len) {
 }
 
 // the quality threshold in force: the PRIME pass of --if reads its files without it (count_main.cc:289-295 uses mer_counter there)
-static uint32_t eff_min_qual(const jfgpu_engine* e) { return e->op == JFGPU_OP_PRIME ? 0u : e->p.min_qual; }
+// (a query reads its text as query_from_sequence does, without qualities)
+static uint32_t eff_min_qual(const jfgpu_engine* e) { return e->op == JFGPU_OP_PRIME || e->querying ? 0u : e->p.min_qual; }
 
-// One batch of device-resident text through K0a, K0b, K1 on `stream`.
+// One batch of device-resident text through K0a, K0b, K1 on `stream`.  mode 0: count, 1: route, 3: record exchange, 4: ordered
+// extraction of a query into the buffers e->qb[e->q_cur].
 int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, cudaStream_t stream,
               int mode, uint64_t* route_keys, unsigned long long* route_counts, uint64_t route_cap, uint64_t n_back = 0) {
   if(n == 0) return JFGPU_OK;
@@ -824,6 +838,7 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
     if(rc) return rc;
   }
   const bool shard_send = mode == 3;            // K1 writes region records of the GLOBAL table into the send pool (bank = route_cap)
+  const bool query = mode == 4;
   const uint32_t tile = (part || shard_send ? 1024 : 512) * 32 - HALO;
   const uint64_t n_tiles = (n + tile - 1) / tile;
   rc = ensure_scratch(e, n_tiles);
@@ -854,6 +869,10 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
   const size_t bloom_smem = a.bloom.mode ? (size_t)e->nbytes * 256 * 8 * 2 : 0;
   if(bc_build) { a.lut = nullptr; a.lut_bytes = 0; a.hash_fast = 0; }
   a.route_keys = route_keys; a.route_counts = route_counts; a.route_cap = route_cap; a.shard_bits = e->shard_bits;
+  if(query) {                                   // no hash, no filter: the keys themselves, in input order
+    a.lut = nullptr; a.lut_bytes = 0; a.hash_fast = 0; memset(&a.bloom, 0, sizeof(a.bloom));
+    a.q_keys = e->qb[e->q_cur].keys.as<uint64_t>(); a.q_cnt = e->qb[e->q_cur].cnt.as<uint32_t>(); a.q_tile_cap = tile;
+  }
   PartDev pd = shard_send ? shard_send_dev(e, (int)route_cap) : part_dev(e);
   auto launch = [&](auto kern, int nth, size_t smem, bool one_per_sm) -> int {
     cudaError_t c = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -865,6 +884,7 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
     // (sharded counting leaves a few SMs to the collective that runs beside K1)
     const int sms = shard_send && e->n_sm > 32 ? e->n_sm - (int)SHARD_RESERVED_SMS : e->n_sm;
     const int grid = (int)std::min<uint64_t>(n_tiles, (uint64_t)sms * per_sm);
+    if(query) { kern<<<grid, nth, smem, stream>>>(a, pd); return JFGPU_OK; }     // (the counting statistics leave a query out)
     if(e->kev_used + 2 > e->kev.size()) { cudaEvent_t a0, a1; cudaEventCreate(&a0); cudaEventCreate(&a1); e->kev.push_back(a0); e->kev.push_back(a1); }
     cudaEventRecord(e->kev[e->kev_used], stream);
     kern<<<grid, nth, smem, stream>>>(a, pd);
@@ -889,6 +909,7 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
       if(kw == 1 && fast) return launch(extract_kernel<1, sb, 2, 1024, true, 6>, 1024, count_smem_bytes<1024>(a.lut_bytes, ps.stage_bytes, 0, true), true);
       return launch(extract_kernel<kw, sb, 2, 1024, false>, 1024, count_smem_bytes<1024>(a.lut_bytes, ps.stage_bytes, bloom_smem), true);
     }
+    if(query) return launch(extract_kernel<kw, 64, 3, 512, false>, 512, count_smem_bytes<512>(0, 0, 0), false);
     if(mode == 1) return launch(extract_kernel<kw, sb, 1, 512, false>, 512, count_smem_bytes<512>(a.lut_bytes, 0, bloom_smem), false);
     return launch(extract_kernel<kw, sb, 0, 512, false>, 512, count_smem_bytes<512>(a.lut_bytes, 0, bloom_smem), false);
   });
@@ -1364,6 +1385,16 @@ void jfgpu_destroy(jfgpu_handle e) {
     if(e->ev_done[i]) cudaEventDestroy(e->ev_done[i]);
   }
   e->nlA.free(); e->nlB.free(); e->cntA.free(); e->cntB.free(); e->tstate.free();
+  for(int i = 0; i < 2; ++i) {
+    jfgpu_engine::QueryBufs& q = e->qb[i];
+    q.keys.free(); q.vals.free(); q.cnt.free(); q.off.free(); q.out.free();
+    if(q.h_off) cudaFreeHost(q.h_off);
+    if(q.h_cnt) cudaFreeHost(q.h_cnt);
+    if(q.ev_front) cudaEventDestroy(q.ev_front);
+    if(q.ev_fmt) cudaEventDestroy(q.ev_fmt);
+    if(e->q_host[i]) cudaFreeHost(e->q_host[i]);
+    if(e->ev_qcopy[i]) cudaEventDestroy(e->ev_qcopy[i]);
+  }
   if(e->h_stats) cudaFreeHost(e->h_stats);
   if(e->h_watch) cudaFreeHost(e->h_watch);
   for(int i = 0; i < 2; ++i) if(e->ev_watch[i]) cudaEventDestroy(e->ev_watch[i]);
@@ -1454,6 +1485,21 @@ static size_t fastq_record_prefix(const char* p, size_t len, uint32_t lines_mod4
   return best;
 }
 
+// Length of the next batch of host text at `off`, at most `cap` bytes: it never ends on '\r' unless the data ends there (the
+// device looks one byte ahead), and with `qfastq` (-Q on FASTQ) only behind a complete record (e->q_lines follows).
+static int next_batch_len(jfgpu_engine* e, const char* bytes, size_t off, size_t n, size_t cap, bool qfastq, size_t* out) {
+  size_t len = cap;
+  if(off + len < n) { size_t l2 = len; while(l2 > 1 && bytes[off + l2 - 1] == '\r') --l2; if(l2 > 1) len = l2; }
+  if(qfastq && off + len < n) {
+    uint32_t l2 = 0;
+    const size_t whole = fastq_record_prefix(bytes + off, len, e->q_lines, &l2);
+    if(whole == 0) return fail(e, JFGPU_ERR_FORMAT, "Invalid fastq file: a record is larger than the staging buffer (or has more than 4 lines)");
+    len = whole; e->q_lines = l2;
+  }
+  *out = len;
+  return JFGPU_OK;
+}
+
 int jfgpu_feed(jfgpu_handle e, const char* bytes, size_t n, uint32_t flags) {
   if(!e) return JFGPU_ERR_ARG;
   cudaSetDevice(e->device);
@@ -1478,15 +1524,9 @@ int jfgpu_feed(jfgpu_handle e, const char* bytes, size_t n, uint32_t flags) {
   cudaEventRecord(e->ev_t0, e->cs);
   size_t off = 0;
   while(off < n) {
-    size_t len = part_cap_len(e, std::min(e->batch_bytes, n - off));
-    // never end a chunk on '\r' unless it is the end of the data: the device looks one byte ahead
-    if(off + len < n) { size_t l2 = len; while(l2 > 1 && bytes[off + l2 - 1] == '\r') --l2; if(l2 > 1) len = l2; }
-    if(qfastq && off + len < n) {              // ... and, under -Q, only on a record boundary
-      uint32_t l2 = 0;
-      const size_t whole = fastq_record_prefix(bytes + off, len, e->q_lines, &l2);
-      if(whole == 0) return fail(e, JFGPU_ERR_FORMAT, "Invalid fastq file: a record is larger than the staging buffer (or has more than 4 lines)");
-      len = whole; e->q_lines = l2;
-    }
+    size_t len = 0;
+    rc = next_batch_len(e, bytes, off, n, part_cap_len(e, std::min(e->batch_bytes, n - off)), qfastq, &len);
+    if(rc) return rc;
     const int s = e->stage_cur;
     // the previous batch that used this staging buffer must be done before it is overwritten
     CUDA_OK(e, cudaEventSynchronize(e->ev_done[s]));
@@ -1936,6 +1976,197 @@ int jfgpu_lookup(jfgpu_handle e, const uint64_t* keys, size_t n, uint64_t* vals)
     if(c != cudaSuccess) rc = fail(e, JFGPU_ERR_CUDA, std::string("lookup: ") + cudaGetErrorString(c));
   }
   dk.free(); dv.free();
+  return rc;
+}
+
+int jfgpu_device_count(void) {
+  int n = 0;
+  if(cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }
+  return n;
+}
+
+int jfgpu_load_records(jfgpu_handle e, const void* records, size_t nbytes, uint32_t counter_len) {
+  if(!e) return JFGPU_ERR_ARG;
+  if(!e->tab.slots.p) return fail(e, JFGPU_ERR_STATE, "this engine holds a Bloom counter, not a hash table");
+  if(e->shard_bits) return fail(e, JFGPU_ERR_STATE, "a database is loaded into a whole table, not a shard");
+  if(counter_len < 1 || counter_len > 8) return fail(e, JFGPU_ERR_ARG, "counter_len must be in [1, 8]");
+  const size_t rec = e->nbytes + counter_len;
+  if(nbytes % rec) return fail(e, JFGPU_ERR_ARG, "the bytes are not a whole number of records (" + std::to_string(e->nbytes) + " key bytes + " + std::to_string(counter_len) + " count bytes each)");
+  if(nbytes && !records) return JFGPU_ERR_ARG;
+  cudaSetDevice(e->device);
+  int rc = jfgpu_finish(e, nullptr);            // (text fed before is counted first)
+  if(rc || nbytes == 0) return rc;
+  const uint64_t n_rec = nbytes / rec;
+  // a slice is at most one group of the failure list (regrow re-inserts what found no slot)
+  const uint64_t slice = std::min<uint64_t>(std::min<uint64_t>(((uint64_t)64 << 20) / rec, e->fail_group), n_rec);
+  uint8_t* h[2] = { nullptr, nullptr };
+  DevBuf raw, keys, counts;
+  bool ok = raw.alloc(slice * rec + 16) == cudaSuccess && keys.alloc(slice * 8 * e->kw) == cudaSuccess && counts.alloc(slice * 8) == cudaSuccess;
+  for(int i = 0; i < 2 && ok; ++i) ok = cudaHostAlloc((void**)&h[i], slice * rec, cudaHostAllocDefault) == cudaSuccess;
+  if(!ok) {
+    cudaGetLastError();
+    rc = fail(e, JFGPU_ERR_NOMEM, "allocation of the load staging buffers failed");
+  }
+  const uint32_t op = e->op;
+  e->op = JFGPU_OP_COUNT;                       // the records' counts are added, whatever the counter is doing
+  const uint8_t* src = (const uint8_t*)records;
+  if(!rc) memcpy(h[0], src, slice * rec);
+  for(uint64_t i = 0, first = 0; first < n_rec && !rc; ++i, first += slice) {
+    const uint64_t m = std::min(slice, n_rec - first);
+    const int b = (int)(i & 1);
+    cudaError_t c = cudaMemcpyAsync(raw.p, h[b], m * rec, cudaMemcpyHostToDevice, e->cs);
+    if(c != cudaSuccess) { rc = fail(e, JFGPU_ERR_CUDA, std::string("load: ") + cudaGetErrorString(c)); break; }
+    const int grid = (int)std::min<uint64_t>((m + 255) / 256, (uint64_t)e->n_sm * 8);
+    if(e->kw == 1) query_decode_kernel<1><<<grid, 256, 0, e->cs>>>(raw.as<uint8_t>(), m, e->nbytes, counter_len, keys.as<uint64_t>(), counts.as<uint64_t>());
+    else query_decode_kernel<2><<<grid, 256, 0, e->cs>>>(raw.as<uint8_t>(), m, e->nbytes, counter_len, keys.as<uint64_t>(), counts.as<uint64_t>());
+    JF_LAUNCHED();
+    rc = insert_keys_into(e, e->tab, keys.as<uint64_t>(), counts.as<uint64_t>(), m, e->cs);
+    if(rc) break;
+    // the next slice goes to the other pinned buffer while this one is inserted (the copy out of it was enqueued before)
+    if(first + m < n_rec) memcpy(h[b ^ 1], src + (first + m) * rec, std::min(slice, n_rec - first - m) * rec);
+    rc = check_after_batches(e);                // (synchronises; a table that is full is doubled, counts and all)
+  }
+  e->op = op;
+  cudaStreamSynchronize(e->cs);
+  raw.free(); keys.free(); counts.free();
+  for(int i = 0; i < 2; ++i) if(h[i]) cudaFreeHost(h[i]);
+  if(rc == JFGPU_ERR_FULL) rc = fail(e, JFGPU_ERR_NOMEM, "the database does not fit in device memory (" + e->err + ")");
+  return rc;
+}
+
+static int query_impl(jfgpu_engine* e, const char* bytes, size_t n, uint32_t flags, jfgpu_sink_fn sink, void* ctx, uint64_t* n_kmers) {
+  int rc = jfgpu_finish(e, nullptr);
+  if(rc) return rc;
+  const unsigned long long fmt_err0 = e->h_stats[STAT_FORMAT_ERR];
+  rc = begin_feed(e, flags, n ? (unsigned char)bytes[0] : -1, e->cs);
+  if(rc) return rc;
+  // batches of at most 16 MB of text: one line per byte at most, up to k + 22 bytes each
+  const uint32_t TILE = 512 * 32 - HALO;
+  const size_t qbatch = std::min<size_t>(e->batch_bytes, (size_t)16 << 20);
+  const uint64_t max_tiles = (qbatch + TILE - 1) / TILE;
+  const size_t PIECE = (size_t)64 << 20;        // bytes handed to the sink at most (whole windows: one window's lines < 1.4 MB)
+  if(e->q_tiles_cap < max_tiles) {
+    CUDA_OK(e, cudaStreamSynchronize(e->cs));
+    for(int i = 0; i < 2; ++i) {
+      jfgpu_engine::QueryBufs& q = e->qb[i];
+      if(q.h_off) { cudaFreeHost(q.h_off); q.h_off = nullptr; }
+      if(q.h_cnt) { cudaFreeHost(q.h_cnt); q.h_cnt = nullptr; }
+      bool ok = q.keys.alloc(max_tiles * TILE * 8 * e->kw) == cudaSuccess && q.vals.alloc(max_tiles * TILE * 8) == cudaSuccess &&
+                q.cnt.alloc(max_tiles * 4) == cudaSuccess && q.off.alloc((max_tiles + 1) * 8) == cudaSuccess &&
+                cudaHostAlloc((void**)&q.h_off, (max_tiles + 1) * 8, cudaHostAllocDefault) == cudaSuccess &&
+                cudaHostAlloc((void**)&q.h_cnt, max_tiles * 4, cudaHostAllocDefault) == cudaSuccess;
+      if(ok && !q.ev_front) ok = cudaEventCreateWithFlags(&q.ev_front, cudaEventDisableTiming) == cudaSuccess &&
+                                 cudaEventCreateWithFlags(&q.ev_fmt, cudaEventDisableTiming) == cudaSuccess;
+      if(ok && !e->q_host[i]) ok = cudaHostAlloc((void**)&e->q_host[i], PIECE, cudaHostAllocDefault) == cudaSuccess &&
+                                   cudaEventCreateWithFlags(&e->ev_qcopy[i], cudaEventDisableTiming) == cudaSuccess;
+      if(!ok) { cudaGetLastError(); return fail(e, JFGPU_ERR_NOMEM, "allocation of the query buffers failed"); }
+    }
+    e->q_tiles_cap = max_tiles;
+  }
+  for(int i = 0; i < 2; ++i) if(!e->stage[i].p) CUDA_OK(e, e->stage[i].alloc(e->batch_bytes + 64));
+  TableDev T = table_dev(e, e->tab);
+  const size_t lut_smem = (size_t)e->nbytes * 256 * 8;
+  // text -> k-mers in order -> counts -> where every window's lines start (enqueued on the compute stream)
+  auto front = [&](int b, size_t off, size_t len) -> int {
+    jfgpu_engine::QueryBufs& q = e->qb[b];
+    const int s = e->stage_cur;
+    CUDA_OK(e, cudaEventSynchronize(e->ev_done[s]));
+    CUDA_OK(e, cudaMemcpyAsync(e->stage[s].p, bytes + off, len, cudaMemcpyHostToDevice, e->hs));
+    CUDA_OK(e, cudaEventRecord(e->ev_copied[s], e->hs));
+    CUDA_OK(e, cudaStreamWaitEvent(e->cs, e->ev_copied[s], 0));
+    e->q_cur = b;
+    int rc2 = run_batch(e, e->stage[s].as<uint8_t>(), len, len, e->cs, 4, nullptr, nullptr, 0);
+    if(rc2) return rc2;
+    CUDA_OK(e, cudaEventRecord(e->ev_done[s], e->cs));
+    e->stage_cur ^= 1;
+    q.n_tiles = (len + TILE - 1) / TILE;
+    const int grid = (int)std::min<uint64_t>(q.n_tiles, (uint64_t)e->n_sm * 8);
+    rc2 = dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int {
+      auto kern = query_lookup_kernel<decltype(KW)::value, decltype(SB)::value>;
+      cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lut_smem);
+      kern<<<grid, QUERY_NTH, lut_smem, e->cs>>>(T, e->tab.lut.as<uint64_t>(), e->nbytes, q.keys.as<uint64_t>(), q.cnt.as<uint32_t>(), TILE,
+                                                  q.n_tiles, e->k, 0, q.vals.as<uint64_t>(), q.off.as<unsigned long long>());
+      return JFGPU_OK;
+    });
+    if(rc2) return rc2;
+    JF_LAUNCHED();
+    query_scan_kernel<<<1, 1024, 0, e->cs>>>(q.off.as<unsigned long long>(), q.n_tiles); JF_LAUNCHED();
+    CUDA_OK(e, cudaGetLastError());
+    CUDA_OK(e, cudaMemcpyAsync(q.h_off, q.off.p, (q.n_tiles + 1) * 8, cudaMemcpyDeviceToHost, e->cs));
+    CUDA_OK(e, cudaMemcpyAsync(q.h_cnt, q.cnt.p, q.n_tiles * 4, cudaMemcpyDeviceToHost, e->cs));
+    CUDA_OK(e, cudaEventRecord(q.ev_front, e->cs));
+    return JFGPU_OK;
+  };
+  uint64_t lines = 0;
+  size_t off = 0, len = 0;
+  if(n) { rc = next_batch_len(e, bytes, 0, n, std::min(qbatch, n), false, &len); if(!rc) rc = front(0, 0, len); }
+  for(int b = 0; off < n && !rc; b ^= 1) {
+    jfgpu_engine::QueryBufs& q = e->qb[b];
+    CUDA_OK(e, cudaEventSynchronize(q.ev_front));
+    const uint64_t total = q.h_off[q.n_tiles];
+    if(q.out.bytes < total) CUDA_OK(e, q.out.alloc(total + (total >> 3)));
+    if(total) {
+      const int grid = (int)std::min<uint64_t>(q.n_tiles, (uint64_t)e->n_sm * 8);
+      if(e->kw == 1) query_format_kernel<1><<<grid, QUERY_NTH, 0, e->cs>>>(q.keys.as<uint64_t>(), q.vals.as<uint64_t>(), q.cnt.as<uint32_t>(), TILE, 0, q.n_tiles, q.off.as<unsigned long long>(), e->k, q.out.as<uint8_t>());
+      else query_format_kernel<2><<<grid, QUERY_NTH, 0, e->cs>>>(q.keys.as<uint64_t>(), q.vals.as<uint64_t>(), q.cnt.as<uint32_t>(), TILE, 0, q.n_tiles, q.off.as<unsigned long long>(), e->k, q.out.as<uint8_t>());
+      JF_LAUNCHED();
+      CUDA_OK(e, cudaGetLastError());
+    }
+    CUDA_OK(e, cudaEventRecord(q.ev_fmt, e->cs));
+    for(uint64_t t = 0; t < q.n_tiles; ++t) lines += q.h_cnt[t];
+    // the next batch is extracted and looked up while the lines of this one go out
+    off += len;
+    if(off < n) {
+      rc = next_batch_len(e, bytes, off, n, std::min(qbatch, n - off), false, &len);
+      if(!rc) rc = front(b ^ 1, off, len);
+      if(rc) break;
+    }
+    // pieces of whole windows, copied through two pinned buffers: piece j+1 is copied while the sink takes piece j
+    std::vector<std::pair<uint64_t, uint64_t>> pieces;          // byte ranges of the batch's output
+    for(uint64_t t = 0; t < q.n_tiles; ) {
+      uint64_t u = t + 1;
+      while(u < q.n_tiles && q.h_off[u + 1] - q.h_off[t] <= PIECE) ++u;
+      if(q.h_off[u] > q.h_off[t]) pieces.push_back(std::make_pair(q.h_off[t], q.h_off[u] - q.h_off[t]));
+      t = u;
+    }
+    CUDA_OK(e, cudaStreamWaitEvent(e->hs, q.ev_fmt, 0));
+    auto copy = [&](size_t j) -> int {
+      CUDA_OK(e, cudaMemcpyAsync(e->q_host[j & 1], q.out.as<uint8_t>() + pieces[j].first, pieces[j].second, cudaMemcpyDeviceToHost, e->hs));
+      CUDA_OK(e, cudaEventRecord(e->ev_qcopy[j & 1], e->hs));
+      return JFGPU_OK;
+    };
+    if(!pieces.empty()) rc = copy(0);
+    for(size_t j = 0; j < pieces.size() && !rc; ++j) {
+      if(j + 1 < pieces.size()) { rc = copy(j + 1); if(rc) break; }
+      CUDA_OK(e, cudaEventSynchronize(e->ev_qcopy[j & 1]));
+      if(sink(ctx, e->q_host[j & 1], pieces[j].second) != 0) rc = fail(e, JFGPU_ERR_SINK, "query sink failed");
+    }
+  }
+  CUDA_OK(e, cudaStreamSynchronize(e->cs));
+  CUDA_OK(e, cudaStreamSynchronize(e->hs));
+  if(rc) return rc;
+  if(n_kmers) *n_kmers = lines;
+  rc = read_stats(e);
+  if(rc) return rc;
+  if(e->h_stats[STAT_FORMAT_ERR] != fmt_err0) {         // (the counter is put back: the table's own text had no such error)
+    CUDA_OK(e, cudaMemcpyAsync(e->stats.as<unsigned long long>() + STAT_FORMAT_ERR, &fmt_err0, 8, cudaMemcpyHostToDevice, e->cs));
+    CUDA_OK(e, cudaStreamSynchronize(e->cs));
+    e->h_stats[STAT_FORMAT_ERR] = fmt_err0;
+    end_feed(e, JFGPU_FILE_END, e->cs);
+    return fail(e, JFGPU_ERR_FORMAT, "Invalid fastq sequence (the device parser reads 4-line FASTQ records: '@' header, sequence, '+', qualities)");
+  }
+  return end_feed(e, flags, e->cs);
+}
+
+int jfgpu_query(jfgpu_handle e, const char* bytes, size_t n, uint32_t flags, jfgpu_sink_fn sink, void* ctx, uint64_t* n_kmers) {
+  if(!e || !sink || (n && !bytes)) return JFGPU_ERR_ARG;
+  if(n_kmers) *n_kmers = 0;
+  if(!e->tab.slots.p) return fail(e, JFGPU_ERR_STATE, "this engine holds a Bloom counter, not a hash table");
+  if(e->shard_bits) return fail(e, JFGPU_ERR_STATE, "a query needs the whole table, not a shard");
+  cudaSetDevice(e->device);
+  e->querying = true;
+  const int rc = query_impl(e, bytes, n, flags, sink, ctx, n_kmers);
+  e->querying = false;
   return rc;
 }
 

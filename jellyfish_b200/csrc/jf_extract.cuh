@@ -487,10 +487,9 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
 
     // ---- phase E: thread c owns stream word PW + c: the k-mers ending at its 32 symbols ----
     const uint32_t n_words = (nsym + 31) / 32;
-    // (FAST: every thread makes exactly one trip, with an empty mask if it owns no word -- the ring passes below are block-wide)
-    for(uint32_t c = tid; c < (FAST ? (uint32_t)NTH : n_words); c += NTH) {
+    // which of the 32 end positions of stream word PW + c carry a k-mer: inside [idx0, nsym), no reset among the last k symbols
+    auto kmer_mask = [&](const uint32_t c) -> uint32_t {
       const uint32_t W = PW + c;
-      // which of the 32 end positions carry a k-mer: inside [idx0, nsym), no reset among the last k symbols
       const int lo_i = (int)idx0 - (int)(32 * c), hi_i = (int)nsym - (int)(32 * c);
       uint32_t vmask = low_mask32((uint32_t)(hi_i > 32 ? 32 : hi_i)) & ~low_mask32((uint32_t)(lo_i < 0 ? 0 : (lo_i > 32 ? 32 : lo_i)));
       {
@@ -516,6 +515,35 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
           vmask &= ~(uint32_t)(x >> 32);
         }
       }
+      return vmask;
+    };
+    // MODE 3: the rank of this thread's first k-mer in the window (exclusive scan of the popcounts of the masks; the window
+    // holds at most NTH stream words, so thread c owns word c); the window's count goes to q_cnt[t]
+    uint32_t q_rank = 0;
+    if constexpr(MODE == 3) {
+      const uint32_t pc = (uint32_t)tid < n_words ? __popc(kmer_mask(tid)) : 0u;
+      uint32_t qinc = pc;
+#pragma unroll
+      for(int o = 1; o < 32; o <<= 1) {
+        const uint32_t up = __shfl_up_sync(0xffffffffu, qinc, o);
+        if(lane >= o) qinc += up;
+      }
+      if(lane == 31) sm.warp_cnt[warp] = qinc;
+      __syncthreads();
+      uint32_t g = lane < NW ? sm.warp_cnt[lane] : 0u;
+#pragma unroll
+      for(int o = 1; o < NW; o <<= 1) {
+        const uint32_t up = __shfl_up_sync(0xffffffffu, g, o);
+        if(lane >= o) g += up;
+      }
+      const uint32_t wo = warp ? __shfl_sync(0xffffffffu, g, warp - 1) : 0u;
+      q_rank = wo + qinc - pc;
+      if(tid == NTH - 1) a.q_cnt[t] = q_rank + pc;
+    }
+    // (FAST: every thread makes exactly one trip, with an empty mask if it owns no word -- the ring passes below are block-wide)
+    for(uint32_t c = tid; c < (FAST ? (uint32_t)NTH : n_words); c += NTH) {
+      const uint32_t W = PW + c;
+      uint32_t vmask = kmer_mask(c);
       if(c >= n_words) vmask = 0;
       if(!FAST && !vmask) continue;
       ls.kmers += __popc(vmask);
@@ -618,6 +646,12 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
           if(!((vm8 >> j) & 1u)) continue;
           uint64_t key[KW];
           kmer_at(j, key);
+          if constexpr(MODE == 3) {        // input order: the k-mers ending in front of this one in the window come first
+            const uint64_t at = (uint64_t)t * a.q_tile_cap + q_rank + __popc(vmask & low_mask32(8u * o + j));
+#pragma unroll
+            for(int q = 0; q < KW; ++q) a.q_keys[at * KW + q] = key[q];
+            continue;
+          }
           if(a.bloom.mode) {
             const uint64_t h1 = gf2_hash<KW>(bl1, key, (int)a.nbytes), h2 = gf2_hash<KW>(bl2, key, (int)a.nbytes);
             if(a.bloom.mode == BLOOM_COUNT) { bloom_count(a.bloom, h1, h2); ls.inserted++; continue; }   // `jellyfish bc`: no table
@@ -691,7 +725,8 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
     for(uint32_t p = tid; p < pd.P; p += NTH) { my_chunk[p] = st_chunk[p]; my_fill[p] = min(FAST ? (st_cnt[p] & 0xFFFFu) : st_cnt[p], pd.chunk_recs); }
   }
 
-  // ---- statistics: one atomic per counter per CTA ----
+  // ---- statistics: one atomic per counter per CTA (a query leaves them alone) ----
+  if constexpr(MODE == 3) return;
   unsigned long long v[4] = { ls.kmers, ls.inserted, ls.distinct, ls.reprobes };
 #pragma unroll
   for(int q = 0; q < 4; ++q) {

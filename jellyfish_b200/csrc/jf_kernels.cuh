@@ -4,7 +4,8 @@
 //   K0b tile_state_kernel   parser state at the start of every staged window
 //   K1  extract_kernel      (jf_extract.cuh) fused: TMA-staged text window -> word-parallel classification -> packed symbol
 //                           streams -> canonical k-mers -> GF(2) hash -> CAS insert (MODE 0), bucket by owning shard
-//                           (MODE 1) or compact region records appended to per-CTA chunk lists (MODE 2)
+//                           (MODE 1), compact region records appended to per-CTA chunk lists (MODE 2), or the keys
+//                           themselves in input order, per window (MODE 3, `query -s`; jf_query.cuh takes it from there)
 //   K2  win_* kernels       (jf_window.cuh) region records -> table, one shared-memory window at a time;
 //       insert_chunks*      the L2 form of the same for slot widths the window form does not cover
 //   K2' insert_keys_kernel  packed keys -> hash -> insert (multi-GPU receive side, regrow, spilled records)
@@ -198,6 +199,11 @@ struct CountArgs {
   uint64_t       n_back;        // bytes readable in front of `in` (the line a window starts in may begin there)
   uint64_t       prow[8];
   BloomDev       bloom;         // filter in front of the table (mode BLOOM_NONE: nothing)
+  // ordered extraction (MODE 3, `query -s`): the k-mers of window t, in input order, at q_keys[(t*q_tile_cap + i)*KW],
+  // i < q_cnt[t]
+  uint64_t*      q_keys;
+  uint32_t*      q_cnt;
+  uint32_t       q_tile_cap;
 };
 
 // the Bloom counter as `jellyfish bc` writes it (bloom_counter2.hpp:34-36: five base-3 digits per byte) from the two-bit form
@@ -963,6 +969,32 @@ __global__ void __launch_bounds__(256) collect_kernel(const CollectArgs a) {
 // ---------------------------------------------------------------------------------------
 // K5: lookups / histogram straight from the resident table
 // ---------------------------------------------------------------------------------------
+// array::get_val_for_key (large_hash_array.hpp:384-405): the count of `key` (hashed to `pos`), counter carries included;
+// 0 when the key is absent or another shard owns it.  Shared by lookup_kernel and query_lookup_kernel (jf_query.cuh).
+template<int KW, int SB>
+__device__ __forceinline__ uint64_t table_get(const TableDev& T, const uint64_t (&key)[KW], uint64_t pos, uint32_t shard_bits) {
+  const uint32_t owner = shard_bits ? (uint32_t)(pos >> (T.lsize - shard_bits)) : 0u;
+  if(owner != T.shard_index) return 0;
+  const u128 want = key_high<KW>(key, T.lsize);
+  const uint64_t base = pos & T.local_mask;
+  uint64_t idx = base;
+  for(uint32_t r = 0; r <= T.max_reprobe; ++r) {
+    u128 high; uint32_t rp; uint64_t cnt;
+    if(!slot_decode<SB>(T, idx, high, rp, cnt)) break;          // empty slot ends the probe sequence
+    if(rp == r && high.lo == want.lo && high.hi == want.hi) {
+      const uint32_t cb = (SB == 128) ? (64 - (T.fbits > 64 ? T.fbits - 64 : 0)) : (SB - T.fbits);
+      const uint64_t carries = T.stats[STAT_OVERFLOWED] ? ovf_get(T, idx) : 0;
+      if(carries) {
+        if(cb >= 64 || (carries >> (64 - cb)) != 0) cnt = ~0ull;
+        else { uint64_t add = carries << cb; cnt = (cnt + add < cnt) ? ~0ull : cnt + add; }
+      }
+      return cnt;
+    }
+    idx = base + tri(r + 1);
+  }
+  return 0;
+}
+
 template<int KW, int SB>
 __global__ void __launch_bounds__(256) lookup_kernel(TableDev T, const uint64_t* __restrict__ lut_g, uint32_t nbytes,
                                                      const uint64_t* __restrict__ keys, uint64_t n, uint64_t* __restrict__ vals,
@@ -976,29 +1008,7 @@ __global__ void __launch_bounds__(256) lookup_kernel(TableDev T, const uint64_t*
 #pragma unroll
     for(int q = 0; q < KW; ++q) key[q] = keys[i * KW + q];
     const uint64_t pos = gf2_hash<KW>(lut, key, (int)nbytes);
-    uint64_t res = 0;
-    const uint32_t owner = shard_bits ? (uint32_t)(pos >> (T.lsize - shard_bits)) : 0u;
-    if(owner == T.shard_index) {
-      const u128 want = key_high<KW>(key, T.lsize);
-      const uint64_t base = pos & T.local_mask;
-      uint64_t idx = base;
-      for(uint32_t r = 0; r <= T.max_reprobe; ++r) {
-        u128 high; uint32_t rp; uint64_t cnt;
-        if(!slot_decode<SB>(T, idx, high, rp, cnt)) break;          // empty slot ends the probe sequence
-        if(rp == r && high.lo == want.lo && high.hi == want.hi) {
-          const uint32_t cb = (SB == 128) ? (64 - (T.fbits > 64 ? T.fbits - 64 : 0)) : (SB - T.fbits);
-          const uint64_t carries = T.stats[STAT_OVERFLOWED] ? ovf_get(T, idx) : 0;
-          if(carries) {
-            if(cb >= 64 || (carries >> (64 - cb)) != 0) cnt = ~0ull;
-            else { uint64_t add = carries << cb; cnt = (cnt + add < cnt) ? ~0ull : cnt + add; }
-          }
-          res = cnt;
-          break;
-        }
-        idx = base + tri(r + 1);
-      }
-    }
-    vals[i] = res;
+    vals[i] = table_get<KW, SB>(T, key, pos, shard_bits);
   }
 }
 

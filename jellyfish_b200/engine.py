@@ -233,6 +233,64 @@ class HashCounter(object):
 
     __getitem__ = get
 
+    def load_records(self, body, counter_len):
+        """Add the records of a binary/sorted body (bytes, or a pointer/size pair in host memory): ceil(2k/8) key bytes
+        then counter_len count bytes each."""
+        if isinstance(body, tuple):
+            ptr, n = body
+        else:
+            buf = bytes(body)
+            ptr, n = C.cast(C.c_char_p(buf), C.c_void_p), len(buf)
+        self._check(self._lib.jfgpu_load_records(self._h, ptr, n, counter_len))
+
+    def query_text(self, data, begin=True, end=True, sink=None):
+        """query_from_sequence (query_main.cc:45-51): the line "MER COUNT\n" for every k-mer of a buffer of FASTA / FASTQ
+        text, in input order.  Returns the lines as bytes without a sink; with one, calls sink(bytes) with whole lines
+        ("discard": the lines stay in the engine's pinned buffer) and returns the number of lines.  `query_bytes` is then
+        the size of the output."""
+        flags = (L.FILE_BEGIN if begin else 0) | (L.FILE_END if end else 0)
+        if isinstance(data, tuple):
+            ptr, n = data
+        else:
+            buf = bytes(data)
+            ptr, n = C.cast(C.c_char_p(buf), C.c_void_p), len(buf)
+        chunks = []
+
+        self.query_bytes = 0
+
+        def _sink(ctx, p, nb):
+            self.query_bytes += nb
+            if sink == "discard":
+                return 0
+            out = C.string_at(p, nb)
+            if sink is None:
+                chunks.append(out)
+            else:
+                sink(out)
+            return 0
+
+        cb = L.SINK_FN(_sink)
+        nk = C.c_uint64(0)
+        self._check(self._lib.jfgpu_query(self._h, ptr, n, flags, cb, None, C.byref(nk)))
+        return b"".join(chunks) if sink is None else nk.value
+
+    def query_files(self, paths, sink, chunk=64 << 20):
+        """`query -s` over a list of files: sink(bytes) gets the lines of every k-mer, file after file; returns the number
+        of lines."""
+        n = 0
+        for path in paths:
+            with open(path, "rb") as f:
+                first = True
+                cur = f.read(chunk)
+                while True:
+                    nxt = f.read(chunk) if cur else b""
+                    n += self.query_text(cur, begin=first, end=not nxt, sink=sink)
+                    first = False
+                    if not nxt:
+                        break
+                    cur = nxt
+        return n
+
     def histogram(self, n_bins=10002):
         hist = (C.c_uint64 * n_bins)()
         self._check(self._lib.jfgpu_histogram(self._h, hist, n_bins))
@@ -357,6 +415,41 @@ class BloomCounter(object):
                 return 0
             cb = L.SINK_FN(_sink)
             self.hc._check(self.hc._lib.jfgpu_bloom_dump(self.hc._h, cb, None))
+
+
+def read_header(path):
+    """-> (header dict, offset of the body) of a jellyfish file (generic_file_header.hpp:58-86)."""
+    with open(path, "rb") as f:
+        head = f.read(9)
+        hlen = int(head)
+        return json.loads(f.read(hlen).rstrip(b"\0").decode()), 9 + hlen
+
+
+def load_database(path, device=0, size=None, max_batch_bytes=0):
+    """A binary/sorted database (`jellyfish count` output) as a HashCounter resident on `device`: get_many, histogram,
+    dump_records, query_text work on it.  The table gets its own hash matrix and at least twice as many slots as the
+    file has records (`size` overrides that; the table doubles when it fills up, counts and all)."""
+    hdr, off = read_header(path)
+    if hdr.get("format") != "binary/sorted":
+        raise JellyfishError(L.ERR_FORMAT, "Unsupported format '%s'. Must be a binary list." % hdr.get("format"))
+    k = hdr["key_len"] // 2
+    rec = (hdr["key_len"] + 7) // 8 + hdr["counter_len"]
+    n_rec = (os.path.getsize(path) - off) // rec
+    hc = HashCounter(size or max(2 * n_rec, 2), 7, k=k, canonical=hdr.get("canonical", False), device=device,
+                     max_batch_bytes=max_batch_bytes)
+    try:
+        piece = max((256 << 20) // rec, 1) * rec
+        with open(path, "rb") as f:
+            f.seek(off)
+            left = n_rec * rec
+            while left:
+                data = f.read(min(piece, left))
+                hc.load_records(data, hdr["counter_len"])
+                left -= len(data)
+    except Exception:
+        hc.close()
+        raise
+    return hc
 
 
 def write_header(f, header):

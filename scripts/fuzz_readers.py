@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Differential fuzz of the host-side readers of jellyfish-b200 (dump, histo, stats, query, merge: plain
-CPU code in jellyfish_b200/csrc/host/jf_cli.cc) against the reference's own tools, on random databases
-written by the reference's `count`. Build-container tool (needs oracle/_ref/jellyfish).
+"""Differential fuzz of the readers of jellyfish-b200 (dump, histo, stats, query, merge: plain CPU code in
+jellyfish_b200/csrc/host/jf_cli.cc, except `query -s`, which runs on the GPU where there is one) against the
+reference's own tools, on random databases written by the reference's `count` (needs oracle/_ref/jellyfish).
     python scripts/fuzz_readers.py [N] [SEED]
 """
 import os
