@@ -76,7 +76,10 @@ typedef struct {
                               (0 = default 256); tests use 1 to exercise that path on small tables */
   uint32_t k2_mode;        /* how the staged records reach the table (K2): 0 = default (shared-memory window
                               insert where the geometry allows it, else the L2 kernels), 1 = L2 kernels only,
-                              2 = the generic L2 kernel only (no 32-bit specialisation); for tests/benchmarks */
+                              2 = the generic L2 kernel only (no 32-bit specialisation), 3 = the window insert with
+                              every group placed by the exact two-pass regroup (the fall-back of a window bucket
+                              that overflows), 4 = the window insert with buckets of no slack, so that nearly every
+                              group overflows one and falls back; for tests/benchmarks */
   uint32_t region_mb;      /* target size of a table region of the region-by-region insertion (0 = default 64); regions are made smaller when that lets a record fit 4 bytes */
   uint32_t bloom_counter;  /* 1: this engine builds a Bloom counter instead of a hash table -- `jellyfish bc`
                               (sub_commands/bc_main.cc:84-161): bf_size = expected number of k-mers (-s), bf_fp =
@@ -133,7 +136,9 @@ typedef struct {
   uint64_t count_kernel_launches;
   double   seconds_drain;  /* device time of the region-by-region insertion passes (CUDA events) */
   double   seconds_win_hist, seconds_win_scatter, seconds_win_insert;   /* of which: the window kernels of K2 (jf_window.cuh),
-                              CUDA events around their launches; insert includes the deferred-record kernel */
+                              CUDA events around their launches.  scatter: the bucket pass and the run starts; hist: the
+                              exact placement of the groups that overflowed a window bucket (0 when none did); insert
+                              includes the deferred-record kernel */
 } jfgpu_stats;
 
 /* -- life cycle: hash_counter ctor / dtor (hash_counter.hpp:50-68) ------------------ */

@@ -82,10 +82,11 @@ struct Table {
 
 struct PartState {
   uint32_t P = 0, region_bits = 0, rec_bytes = 0, cap = 0, flush_min = 0, stage_bytes = 0, n_chunks = 0, margin = 0, arena_chunks = 0, n_arenas = 0;
-  DevBuf pool, dir, order, pool_next, cta_chunk, cta_fill, spill_keys, spill_counts, spill_n, hist, start, cursor, unit_cursor;
+  DevBuf pool, dir, order, pool_next, cta_chunk, cta_fill, spill_keys, spill_counts, spill_n, hist, start, cursor, unit_cursor;   // (hist: region_recs)
   uint64_t spill_cap = 0;
   // window form of K2 (jf_window.cuh)
   DevBuf w_start, w_cursor, w_cnt, w_rec, w_def_pos[2], w_def_high[2], w_def_n;    // (two deferred lists, w_def_n: their two lengths)
+  DevBuf w_flag;                 // [PMAX] overflow flag of every group of a drain (a group that needed the exact placement)
   uint64_t w_rec_cap = 0, w_def_cap = 0;
   uint64_t bound_chunks = 0;     // host-side upper bound of the chunks in use in any one arena
   bool pending = false;          // records sit in the pool
@@ -445,7 +446,7 @@ int part_alloc(jfgpu_engine* e) {
             ps.order.alloc((size_t)ps.n_chunks * 4) == cudaSuccess && ps.pool_next.alloc(((size_t)ps.n_arenas + 2) * 4) == cudaSuccess &&
             ps.cta_chunk.alloc((size_t)e->n_sm * PMAX * 4) == cudaSuccess && ps.cta_fill.alloc((size_t)e->n_sm * PMAX * 4) == cudaSuccess &&
             ps.spill_keys.alloc(ps.spill_cap * 8 * e->kw) == cudaSuccess && ps.spill_counts.alloc(ps.spill_cap * 8) == cudaSuccess &&
-            ps.spill_n.alloc(8) == cudaSuccess && ps.hist.alloc(PMAX * 4) == cudaSuccess && ps.start.alloc(PMAX * 4) == cudaSuccess &&
+            ps.spill_n.alloc(8) == cudaSuccess && ps.hist.alloc(PMAX * 12) == cudaSuccess && ps.start.alloc(PMAX * 4) == cudaSuccess &&
             ps.cursor.alloc(PMAX * 4) == cudaSuccess && ps.unit_cursor.alloc(8) == cudaSuccess;
   if(!ok) { cudaGetLastError(); return fail(e, JFGPU_ERR_NOMEM, "device allocation of the record pool failed"); }
   CUDA_OK(e, cudaMemsetAsync(ps.pool_next.p, 0, ps.pool_next.bytes, e->cs));
@@ -458,11 +459,14 @@ int part_alloc(jfgpu_engine* e) {
   return JFGPU_OK;
 }
 
+// records per region (chunk_hist_kernel), behind the chunk counts in `hist`
+static unsigned long long* region_recs(PartState& ps) { return reinterpret_cast<unsigned long long*>(ps.hist.as<uint32_t>() + PMAX); }
+
 void part_release(jfgpu_engine* e) {
   PartState& ps = e->part;
   ps.pool.free(); ps.dir.free(); ps.order.free(); ps.pool_next.free(); ps.cta_chunk.free(); ps.cta_fill.free();
   ps.spill_keys.free(); ps.spill_counts.free(); ps.spill_n.free(); ps.hist.free(); ps.start.free(); ps.cursor.free(); ps.unit_cursor.free();
-  ps.w_start.free(); ps.w_cursor.free(); ps.w_cnt.free(); ps.w_rec.free(); ps.w_def_n.free();
+  ps.w_start.free(); ps.w_cursor.free(); ps.w_cnt.free(); ps.w_rec.free(); ps.w_def_n.free(); ps.w_flag.free();
   for(int i = 0; i < 2; ++i) { ps.w_def_pos[i].free(); ps.w_def_high[i].free(); }
   ps.w_rec_cap = ps.w_def_cap = 0;
   ps.n_chunks = 0; ps.arena_chunks = 0; ps.n_arenas = 0; ps.pending = false;
@@ -493,18 +497,26 @@ static cudaEvent_t win_event(jfgpu_engine* e, cudaStream_t st) {
   cudaEventRecord(ev, st);
   return ev;
 }
-// fold the event quadruples of the finished drain into win_ms (the stream must be idle)
-static void resolve_win_events(jfgpu_engine* e) {
-  for(size_t i = 0; i + 3 < e->wev_used; i += 4)
+// Fold the event quadruples of the finished drain into win_ms (the stream must be idle).  Quadruple j belongs to the drain's
+// j-th group with records: bucket pass + scan -> scatter; the exact pass -> hist when that group overflowed a bucket (w_flag[j]),
+// else (a launch that returned at once) scatter; window insert -> insert.
+static void resolve_win_events(jfgpu_engine* e, cudaStream_t st) {
+  const size_t n_groups = e->wev_used / 4;
+  std::vector<uint32_t> flag(n_groups);
+  if(n_groups && (cudaMemcpyAsync(flag.data(), e->part.w_flag.p, n_groups * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+                  cudaStreamSynchronize(st) != cudaSuccess)) cudaGetLastError();
+  for(size_t j = 0; j < n_groups; ++j)
     for(int q = 0; q < 3; ++q) {
       float ms = 0;
-      if(cudaEventElapsedTime(&ms, e->wev[i + q], e->wev[i + q + 1]) == cudaSuccess) e->win_ms[q] += ms; else cudaGetLastError();
+      const int to = q == 0 ? 1 : q == 1 ? (flag[j] ? 0 : 1) : 2;
+      if(cudaEventElapsedTime(&ms, e->wev[4 * j + q], e->wev[4 * j + q + 1]) == cudaSuccess) e->win_ms[to] += ms; else cudaGetLastError();
     }
   e->wev_used = 0;
 }
+// k2_mode 3 and 4 take the window form too (include/jfgpu.h)
 static bool window_enabled(jfgpu_engine* e, const PartDev& pd) {
-  return e->p.k2_mode == 0 && e->op == 0 && e->tab.slot_bits == 32 && pd.rec_bytes == 4 && pd.region_bits > WIN_LG &&
-         pd.region_bits - WIN_LG <= 11 && CHUNK_BYTES == WIN_NTH * 16;
+  return (e->p.k2_mode == 0 || e->p.k2_mode == 3 || e->p.k2_mode == 4) && e->op == 0 && e->tab.slot_bits == 32 && pd.rec_bytes == 4 &&
+         pd.region_bits > WIN_LG && pd.region_bits - WIN_LG <= 11 && CHUNK_BYTES == (WIN_ST_NTH / 2) * 16;
 }
 // Whether a cleared table may stay zero in meaning only until its first drain: that drain takes the window form (plain
 // insertion, no Bloom prefilter) and then writes every slot of [0, local_size), and a deferred probe reaches less than one
@@ -523,7 +535,8 @@ static int window_drain(jfgpu_engine* e, cudaStream_t st, const PartDev& pd, uns
     ps.w_rec_cap = (uint64_t)64 << 20;                       // records per group (256 MB)
     ps.w_def_cap = WIN_DEF_CAP;
     bool ok = ps.w_rec.alloc(ps.w_rec_cap * 4 + 64) == cudaSuccess && ps.w_start.alloc((((size_t)WIN_MAX_G << 11) + 1) * 4) == cudaSuccess &&
-              ps.w_cursor.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_cnt.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_def_n.alloc(16) == cudaSuccess;
+              ps.w_cursor.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_cnt.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_def_n.alloc(16) == cudaSuccess &&
+              ps.w_flag.alloc(PMAX * 4) == cudaSuccess;
     for(int i = 0; i < 2 && ok; ++i) ok = ps.w_def_pos[i].alloc(ps.w_def_cap * 8) == cudaSuccess && ps.w_def_high[i].alloc(ps.w_def_cap * 4) == cudaSuccess;
     if(!ok) { cudaGetLastError(); return fail(e, JFGPU_ERR_NOMEM, "device allocation of the window buffers failed"); }
     CUDA_OK(e, cudaMemsetAsync(ps.w_def_n.p, 0, 16, st));
@@ -553,28 +566,45 @@ static int window_drain(jfgpu_engine* e, cudaStream_t st, const PartDev& pd, uns
     def_wait = -1; zero = false;
     return JFGPU_OK;
   };
-  // first unit of every region (chunk_scan_kernel wrote it), on the host
+  // the groups' overflow flags (k2_mode 3: set from the start, so that every group takes the exact placement)
+  CUDA_OK(e, cudaMemsetAsync(ps.w_flag.p, e->p.k2_mode == 3 ? 1 : 0, PMAX * 4, st));
+  // first unit and records of every region (chunk_scan_kernel, chunk_hist_kernel), on the host
   std::vector<uint32_t> start(pd.P + 1);
+  std::vector<unsigned long long> recs(pd.P);
   CUDA_OK(e, cudaMemcpyAsync(start.data(), ps.start.p, (size_t)pd.P * 4, cudaMemcpyDeviceToHost, st));
+  CUDA_OK(e, cudaMemcpyAsync(recs.data(), region_recs(ps), (size_t)pd.P * 8, cudaMemcpyDeviceToHost, st));
   CUDA_OK(e, cudaStreamSynchronize(st));
   start[pd.P] = n_units;
   for(uint32_t r = 0; r < pd.P; ++r) start[r] = std::min(start[r], n_units);
   uint32_t r0 = 0;
   while(r0 < pd.P && start[r0] < *done) ++r0;
   const size_t scatter_smem = ((size_t)4 * ((size_t)1 << wpr_lg) + (size_t)WIN_ST_UNITS * pd.chunk_recs) * 4;
-  cudaFuncSetAttribute(win_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scatter_smem);
-  // (the runs of a group start on 16-byte boundaries: up to 3 padding records per window)
-  const uint64_t max_units = std::min<uint64_t>((ps.w_rec_cap - ((uint64_t)WIN_MAX_G << 13)) / pd.chunk_recs, careful ? group_units : 0xFFFFFFFFu);
+  cudaFuncSetAttribute(win_scatter_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scatter_smem);
+  cudaFuncSetAttribute(win_scatter_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scatter_smem);
+  // Bucket capacity of a group: m = the largest mean of records per window over its regions.  A window's count is about
+  // Poisson(m) for hashed input; m + 6 sqrt(m) + 16 leaves a window of iid input a chance of order 1e-9 to overflow, i.e.
+  // a fallback to the exact placement about once in two thousand steps of configs[1] (half a million windows).  k2_mode 4
+  // leaves no slack, so nearly every group overflows.  Regions join a group while its buckets fit the group buffer, and
+  // so does its exact layout: the group's records (at most m per window on average) plus up to 3 padding records per
+  // window, since every run starts on a 16-byte boundary.
+  const uint64_t wpr = (uint64_t)1 << wpr_lg;
+  auto bucket_cap = [&](uint64_t m) -> uint64_t {
+    const uint64_t c = e->p.k2_mode == 4 ? m : m + (uint64_t)std::ceil(6.0 * std::sqrt((double)m)) + 16;
+    return (c + 3) & ~(uint64_t)3;
+  };
   uint32_t gi = 0, ng = 0;
   while(r0 < pd.P && *done < n_units) {
     WinDev wd;
     memset(&wd, 0, sizeof(wd));
-    uint32_t G = 0, tiles = 0, stiles = 0;
+    uint32_t G = 0, stiles = 0;
+    uint64_t m = 0, cap = 0;
     while(r0 + G < pd.P && G < WIN_MAX_G) {
       const uint32_t nu = start[r0 + G + 1] - start[r0 + G];
-      if((uint64_t)(start[r0 + G + 1] - start[r0]) > max_units) break;
-      wd.tile_first[G] = tiles; wd.stile_first[G] = stiles; wd.unit_first[G] = start[r0 + G];
-      tiles += (nu + WIN_TILE_UNITS - 1) / WIN_TILE_UNITS;
+      if(careful && start[r0 + G + 1] - start[r0] > group_units) break;
+      const uint64_t m2 = std::max<uint64_t>(m, (recs[r0 + G] + wpr - 1) / wpr), cap2 = bucket_cap(m2);
+      if((G + 1) * wpr * std::max(cap2, m2 + 3) > ps.w_rec_cap) break;
+      m = m2; cap = cap2;
+      wd.stile_first[G] = stiles; wd.unit_first[G] = start[r0 + G];
       stiles += (nu + WIN_ST_UNITS - 1) / WIN_ST_UNITS;
       ++G;
     }
@@ -590,8 +620,9 @@ static int window_drain(jfgpu_engine* e, cudaStream_t st, const PartDev& pd, uns
       JF_LAUNCHED();
       *done = upto; r0 += 1;
     } else {
-      wd.tile_first[G] = tiles; wd.stile_first[G] = stiles; wd.unit_first[G] = start[r0 + G];
-      wd.g0 = r0; wd.G = G; wd.wpr_lg = wpr_lg; wd.n_tiles = tiles;
+      wd.stile_first[G] = stiles; wd.unit_first[G] = start[r0 + G];
+      wd.g0 = r0; wd.G = G; wd.wpr_lg = wpr_lg; wd.n_tiles = stiles; wd.cap = (uint32_t)cap;
+      wd.overflow = ps.w_flag.as<uint32_t>() + e->wev_used / 4;      // (flag j: the drain's j-th group with records, resolve_win_events)
       wd.wstart = ps.w_start.as<uint32_t>(); wd.wcursor = ps.w_cursor.as<uint32_t>(); wd.wcnt = ps.w_cnt.as<uint32_t>();
       wd.wrec = ps.w_rec.as<uint32_t>(); wd.wrec_cap = ps.w_rec_cap;
       const int set = zero ? (int)(ng & 1) : 0;
@@ -601,19 +632,20 @@ static int window_drain(jfgpu_engine* e, cudaStream_t st, const PartDev& pd, uns
       const uint32_t hb = e->tab.fbits - e->tab.rbits;
       // the deferred records, once every slot they can reach holds its value in memory
       auto settle = [&]() {
-        if(!zero) { if(tiles) run_deferred(set); return; }
+        if(!zero) { if(stiles) run_deferred(set); return; }
         e->tab.materialized = (uint64_t)(r0 + G) << pd.region_bits;
         if(def_wait >= 0) run_deferred(def_wait);
-        def_wait = tiles ? set : -1;
+        def_wait = stiles ? set : -1;
       };
       ++ng;
-      if(tiles) {
+      if(stiles) {
         CUDA_OK(e, cudaMemsetAsync(ps.w_cursor.p, 0, ((size_t)G << wpr_lg) * 4, st));
         win_event(e, st);
-        win_hist_kernel<<<tiles, WIN_NTH, 0, st>>>(pd, wd, ps.order.as<uint32_t>(), hb); JF_LAUNCHED();
+        win_scatter_kernel<true><<<stiles, WIN_ST_NTH, scatter_smem, st>>>(pd, wd, ps.order.as<uint32_t>(), hb); JF_LAUNCHED();
         win_scan_kernel<<<1, 1024, 0, st>>>(wd, T.stats); JF_LAUNCHED();
         win_event(e, st);
-        win_scatter_kernel<<<stiles, WIN_ST_NTH, scatter_smem, st>>>(pd, wd, ps.order.as<uint32_t>(), hb); JF_LAUNCHED();
+        win_scatter_kernel<false><<<std::min<uint32_t>(stiles, e->n_sm * 2), WIN_ST_NTH, scatter_smem, st>>>(pd, wd, ps.order.as<uint32_t>(), hb);
+        JF_LAUNCHED();
         win_event(e, st);
         if(e->kw == 1) {
           cudaFuncSetAttribute(win_insert2_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WIN2_SMEM);
@@ -672,8 +704,8 @@ int part_drain(jfgpu_engine* e, cudaStream_t st) {
   if(!e->ev_d0) { cudaEventCreate(&e->ev_d0); cudaEventCreate(&e->ev_d1); }
   cudaEventRecord(e->ev_d0, st);
   close_chunks_kernel<<<g, 256, 0, st>>>(pd, (uint32_t)e->n_sm); JF_LAUNCHED();
-  CUDA_OK(e, cudaMemsetAsync(ps.hist.p, 0, PMAX * 4, st));
-  chunk_hist_kernel<<<g, 256, 0, st>>>(pd, ps.hist.as<uint32_t>()); JF_LAUNCHED();
+  CUDA_OK(e, cudaMemsetAsync(ps.hist.p, 0, PMAX * 12, st));
+  chunk_hist_kernel<<<g, 256, 0, st>>>(pd, ps.hist.as<uint32_t>(), window_enabled(e, pd) ? region_recs(ps) : nullptr); JF_LAUNCHED();
   chunk_scan_kernel<<<1, 1024, 0, st>>>(pd.P, ps.hist.as<uint32_t>(), ps.start.as<uint32_t>(), ps.cursor.as<uint32_t>(), pd.n_units); JF_LAUNCHED();
   chunk_scatter_kernel<<<g, 256, 0, st>>>(pd, ps.cursor.as<uint32_t>(), ps.order.as<uint32_t>()); JF_LAUNCHED();
   CUDA_OK(e, cudaMemsetAsync(ps.unit_cursor.p, 0, 8, st));
@@ -781,7 +813,7 @@ int part_drain(jfgpu_engine* e, cudaStream_t st) {
   cudaEventRecord(e->ev_d1, st);
   cudaStreamSynchronize(st);
   { float ms = 0; if(cudaEventElapsedTime(&ms, e->ev_d0, e->ev_d1) == cudaSuccess) e->drain_ms += ms; else cudaGetLastError(); }
-  resolve_win_events(e);
+  resolve_win_events(e, st);
   ps.pending = false;
   if(rebuilt) { cudaStreamSynchronize(st); old_inv.free(); part_configure(e); if(!e->part.P) part_release(e); }
   ps.bound_chunks = ps.P;

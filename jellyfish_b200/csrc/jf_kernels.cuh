@@ -412,9 +412,14 @@ __global__ void close_chunks_kernel(PartDev pd, uint32_t n_cta) {
     if(c != NO_CHUNK) { pd.dir[c] = make_uint2((uint32_t)(i % pd.P), pd.cta_fill[i]); pd.cta_chunk[i] = NO_CHUNK; pd.cta_fill[i] = 0; }
   }
 }
-__global__ void chunk_hist_kernel(PartDev pd, uint32_t* __restrict__ hist) {
+// chunks per region, and records per region unless `recs` is null (only the window form of K2 sizes its groups by records)
+__global__ void chunk_hist_kernel(PartDev pd, uint32_t* __restrict__ hist, unsigned long long* __restrict__ recs) {
   for(uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < pd.n_chunks; i += gridDim.x * blockDim.x)
-    if(chunk_in_use(pd, i)) atomicAdd(&hist[pd.dir[i].x], 1u);
+    if(chunk_in_use(pd, i)) {
+      const uint2 d = pd.dir[i];
+      atomicAdd(&hist[d.x], 1u);
+      if(recs) atomicAdd(&recs[d.x], (unsigned long long)d.y);
+    }
 }
 __global__ void __launch_bounds__(1024) chunk_scan_kernel(uint32_t P, const uint32_t* __restrict__ hist, uint32_t* __restrict__ start, uint32_t* __restrict__ cursor,
                                                           unsigned int* __restrict__ n_units) {

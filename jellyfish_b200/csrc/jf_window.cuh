@@ -2,9 +2,12 @@
 //
 // The L2 form of K2 (insert_chunks32_kernel) performs ~2 L2 operations per k-mer (first-probe CAS, reprobes,
 // look-ahead loads).  Here the probing happens in shared memory:
-//   win_hist / win_scan / win_scatter  split the 4-byte records of a group of regions by WINDOW
+//   win_scatter<true> / win_scan / win_scatter<false>  split the 4-byte records of a group of regions by WINDOW
 //        (2^WIN_LG slots = 64 KB of 32-bit slots) with a shared-memory staged tile sort, so that each
-//        window's records are contiguous (12 B of traffic per record);
+//        window's records are contiguous (8 B of traffic per record).  The bucket pass puts every window's records
+//        into a bucket of fixed capacity (wd.cap), so it needs no count beforehand; its atomics on the window
+//        cursors leave the exact count of every window behind.  A window that overflows its bucket flags the group,
+//        and only then does the exact pass place the group's records again, at offsets scanned from those counts;
 //   win_insert2  persistent, one CTA per SM, two stages: while the CTA applies the records of one window with
 //        shared-memory CAS/add along the reference's probe sequence pos + i(i+1)/2, the TMA engine brings in the
 //        next window and its records (cp.async.bulk + mbarrier) and writes the previous window back
@@ -28,70 +31,39 @@
 
 namespace jfk {
 
-constexpr uint32_t WIN_TILE_UNITS = 4;             // chunks per partition tile: 8192 records
 constexpr uint32_t WIN_MAX_G = 64;                 // regions per group
 constexpr uint32_t WIN_MAX_WPR = 2048;             // windows per region (region_bits - WIN_LG <= 11)
-constexpr uint32_t WIN_NTH = 512;
 
 struct WinDev {
-  uint32_t g0, G, wpr_lg, n_tiles;
+  uint32_t g0, G, wpr_lg, n_tiles;                 // n_tiles: win_scatter's tiles of the group
+  uint32_t cap;                                    // records per window bucket (a multiple of 4: buckets start on 16-byte boundaries)
   const uint32_t* lazy_win;                        // write-only drain: the table's window states (only WIN_IN_MEMORY windows are loaded); else null
-  uint32_t tile_first[WIN_MAX_G + 1];              // prefix sum of tiles per region of the group (win_hist: WIN_TILE_UNITS chunks)
-  uint32_t stile_first[WIN_MAX_G + 1];             // the same for win_scatter's larger tiles (WIN_ST_UNITS chunks)
+  uint32_t stile_first[WIN_MAX_G + 1];             // prefix sum of win_scatter's tiles (WIN_ST_UNITS chunks) per region of the group
   uint32_t unit_first[WIN_MAX_G + 1];              // first unit (index into `order`) of each region; [G] = end
-  uint32_t* wstart;                                // [(G << wpr_lg) + 1] exclusive offsets into wrec after win_scan
-  uint32_t* wcursor;                               // [G << wpr_lg] counts (win_hist), then write cursors (win_scatter)
+  uint32_t* overflow;                              // the group's flag: some window holds more than `cap` records
+  uint32_t* wstart;                                // [(G << wpr_lg) + 1] offsets into wrec after win_scan
+  uint32_t* wcursor;                               // [G << wpr_lg] counts (bucket pass), then write cursors (exact pass)
   uint32_t* wcnt;                                  // [G << wpr_lg] records per window (win_scan); runs start on 16-byte boundaries
   uint32_t* wrec; uint64_t wrec_cap;               // records grouped by (region, window)
   uint64_t* def_pos; uint32_t* def_high; unsigned long long* def_n; uint64_t def_cap;
 };
-
-__device__ __forceinline__ uint32_t win_region_of_tile(const WinDev& wd, uint32_t tile) {
-  uint32_t r = 0;
-  while(r + 1 < wd.G && wd.tile_first[r + 1] <= tile) ++r;
-  return r;
-}
 
 // first slot of window `task` (= region of the group << wpr_lg | window of the region)
 __device__ __forceinline__ uint64_t win_slot_base(const WinDev& wd, uint32_t region_bits, uint32_t task) {
   return ((uint64_t)(wd.g0 + (task >> wd.wpr_lg)) << region_bits) + ((uint64_t)(task & ((1u << wd.wpr_lg) - 1)) << WIN_LG);
 }
 
-// ---- counts per (region, window) ---------------------------------------------------------------
-__global__ void __launch_bounds__(WIN_NTH) win_hist_kernel(PartDev pd, WinDev wd, const uint32_t* __restrict__ order, uint32_t hb) {
-  __shared__ uint32_t cnt[WIN_MAX_WPR];
-  const uint32_t wpr = 1u << wd.wpr_lg;
-  for(uint32_t i = threadIdx.x; i < wpr; i += WIN_NTH) cnt[i] = 0;
-  __syncthreads();
-  const uint32_t r = win_region_of_tile(wd, blockIdx.x);
-  const uint32_t u0 = wd.unit_first[r] + (blockIdx.x - wd.tile_first[r]) * WIN_TILE_UNITS;
-  const uint32_t u1 = min(u0 + WIN_TILE_UNITS, wd.unit_first[r + 1]);
-  // the loads of the tile's chunks level by level (order -> directory -> records), so that they overlap
-  uint32_t chunk[WIN_TILE_UNITS], n[WIN_TILE_UNITS]; uint4 v[WIN_TILE_UNITS];
-#pragma unroll
-  for(uint32_t j = 0; j < WIN_TILE_UNITS; ++j) chunk[j] = u0 + j < u1 ? __ldg(order + u0 + j) : 0u;
-#pragma unroll
-  for(uint32_t j = 0; j < WIN_TILE_UNITS; ++j) n[j] = u0 + j < u1 ? __ldg(&pd.dir[chunk[j]].y) : 0u;
-#pragma unroll
-  for(uint32_t j = 0; j < WIN_TILE_UNITS; ++j) {
-    v[j] = make_uint4(0, 0, 0, 0);
-    if(threadIdx.x * 4 < n[j]) v[j] = __ldg(reinterpret_cast<const uint4*>(pd.pool + (size_t)chunk[j] * CHUNK_BYTES) + threadIdx.x);
-  }
-#pragma unroll
-  for(uint32_t j = 0; j < WIN_TILE_UNITS; ++j) {
-    const uint32_t i = threadIdx.x * 4;
-    const uint32_t rec[4] = { v[j].x, v[j].y, v[j].z, v[j].w };
-#pragma unroll
-    for(uint32_t q = 0; q < 4; ++q) if(i + q < n[j]) atomicAdd(&cnt[((rec[q] >> hb) >> WIN_LG) & (wpr - 1)], 1u);
-  }
-  __syncthreads();
-  for(uint32_t i = threadIdx.x; i < wpr; i += WIN_NTH) if(cnt[i]) atomicAdd(&wd.wcursor[(r << wd.wpr_lg) + i], cnt[i]);
-}
-
-// ---- exclusive scan of the counts (one CTA) ------------------------------------------------------
+// ---- run starts of the windows (one CTA) --------------------------------------------------------
+// After the bucket pass wcursor holds every window's count.  Group not flagged: window i's run is bucket i.  Flagged: the exact
+// layout, an exclusive scan of the counts, which also sets wcursor to the run starts for the exact pass.
 __global__ void __launch_bounds__(1024) win_scan_kernel(WinDev wd, unsigned long long* __restrict__ stats) {
   __shared__ uint32_t part[1024];
   const uint32_t n = wd.G << wd.wpr_lg;
+  if(*wd.overflow == 0) {
+    for(uint32_t i = threadIdx.x; i < n; i += 1024) { wd.wstart[i] = i * wd.cap; wd.wcnt[i] = wd.wcursor[i]; }
+    if(threadIdx.x == 0) wd.wstart[n] = n * wd.cap;
+    return;
+  }
   const uint32_t per = (n + 1023) / 1024;
   const uint32_t b = threadIdx.x * per, e = min(b + per, n);
   uint32_t s = 0;
@@ -123,22 +95,29 @@ __global__ void __launch_bounds__(1024) win_scan_kernel(WinDev wd, unsigned long
 // coalesced stores.  The GPU retires a bounded number of store transactions per second whatever their size
 // (scripts/micro/scatter_store.cu), so the tile is as large as two resident CTAs per SM allow.  The chunks are read twice
 // (second time from L2) instead of being held in registers across the scan.
+// BUCKETS (the bucket pass, one CTA per tile): the run of window gw goes to bucket gw after what earlier tiles put there;
+// a run that would overflow the bucket is not stored and flags the group.  Either way its length is added to wcursor[gw],
+// so the pass leaves every window's exact count behind.  Once a CTA sees the flag it stores nothing: the group is placed
+// again by the exact pass (!BUCKETS), which returns at once when the flag is clear and otherwise strides over the tiles
+// with a persistent grid, storing every run at the start win_scan gave it.
 constexpr uint32_t WIN_ST_UNITS = 12;
 constexpr uint32_t WIN_ST_NTH = 1024;
 
-__global__ void __launch_bounds__(WIN_ST_NTH, 2) win_scatter_kernel(PartDev pd, WinDev wd, const uint32_t* __restrict__ order, uint32_t hb) {
+template<bool BUCKETS>
+__device__ __forceinline__ void win_scatter_tile(const PartDev& pd, const WinDev& wd, const uint32_t* __restrict__ order, uint32_t hb, uint32_t tile) {
   extern __shared__ __align__(16) uint32_t wsm[];
   const uint32_t wpr = 1u << wd.wpr_lg;
   uint32_t* cnt = wsm; uint32_t* lbase = cnt + wpr; uint32_t* lcur = lbase + wpr; uint32_t* gbase = lcur + wpr;
   uint32_t* stage = gbase + wpr;                   // WIN_ST_UNITS * chunk_recs records
   __shared__ uint32_t warp_tot[WIN_ST_NTH / 32];
   __shared__ uint32_t s_chunk[WIN_ST_UNITS], s_n[WIN_ST_UNITS];
+  __shared__ uint32_t s_skip;
   const uint32_t tid = threadIdx.x;
   for(uint32_t i = tid; i < wpr; i += WIN_ST_NTH) cnt[i] = 0;
   // which region this tile belongs to (tiles are numbered region by region)
   uint32_t r = 0;
-  while(r + 1 < wd.G && wd.stile_first[r + 1] <= blockIdx.x) ++r;
-  const uint32_t u0 = wd.unit_first[r] + (blockIdx.x - wd.stile_first[r]) * WIN_ST_UNITS;
+  while(r + 1 < wd.G && wd.stile_first[r + 1] <= tile) ++r;
+  const uint32_t u0 = wd.unit_first[r] + (tile - wd.stile_first[r]) * WIN_ST_UNITS;
   const uint32_t u1 = min(u0 + WIN_ST_UNITS, wd.unit_first[r + 1]);
   if(tid < WIN_ST_UNITS) {
     uint32_t c = 0, n = 0;
@@ -175,10 +154,21 @@ __global__ void __launch_bounds__(WIN_ST_NTH, 2) win_scatter_kernel(PartDev pd, 
   for(uint32_t i = b; i < min(b + per, wpr); ++i) {
     const uint32_t c = cnt[i];
     lbase[i] = run; lcur[i] = run;
-    gbase[i] = (c ? atomicAdd(&wd.wcursor[(r << wd.wpr_lg) + i], c) : 0u) - run;      // (output position = this + index in the staging buffer)
+    uint32_t at = 0;
+    if(c) {
+      const uint32_t gw = (r << wd.wpr_lg) + i;
+      at = atomicAdd(&wd.wcursor[gw], c);
+      if(BUCKETS) {
+        if(at + c <= wd.cap) at += gw * wd.cap;
+        else { at = (uint32_t)wd.wrec_cap; *(volatile uint32_t*)wd.overflow = 1u; }    // (every store of the run is past wrec_cap)
+      }
+    }
+    gbase[i] = at - run;                           // (output position = this + index in the staging buffer)
     run += c;
   }
+  if(BUCKETS && tid == 0) s_skip = *(volatile uint32_t*)wd.overflow;
   __syncthreads();
+  if(BUCKETS && s_skip) return;
 #pragma unroll
   for(uint32_t it = 0; it < WIN_ST_UNITS / 2; ++it) {
     const uint32_t j = 2 * it + half, n = s_n[j];
@@ -194,6 +184,19 @@ __global__ void __launch_bounds__(WIN_ST_NTH, 2) win_scatter_kernel(PartDev pd, 
     const uint32_t v = stage[i], w = ((v >> hb) >> WIN_LG) & wmask;
     const uint32_t dst = gbase[w] + i;
     if(dst < wd.wrec_cap) wd.wrec[dst] = v;
+  }
+}
+
+template<bool BUCKETS>
+__global__ void __launch_bounds__(WIN_ST_NTH, 2) win_scatter_kernel(PartDev pd, WinDev wd, const uint32_t* __restrict__ order, uint32_t hb) {
+  if constexpr(BUCKETS) {
+    win_scatter_tile<true>(pd, wd, order, hb, blockIdx.x);
+  } else {
+    if(*wd.overflow == 0) return;
+    for(uint32_t t = blockIdx.x; t < wd.n_tiles; t += gridDim.x) {
+      win_scatter_tile<false>(pd, wd, order, hb, t);
+      __syncthreads();                             // (the next tile reuses the shared memory)
+    }
   }
 }
 
