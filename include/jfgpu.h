@@ -51,7 +51,9 @@ enum { JFGPU_OP_COUNT = 0, JFGPU_OP_PRIME = 1, JFGPU_OP_UPDATE = 2 };
  * (sub_commands/count_main_cmdline.yaggo:4-112). */
 typedef struct {
   uint32_t struct_size;    /* sizeof(jfgpu_params), for ABI evolution                */
-  uint32_t k;              /* -m : mer length, 1..64                                  */
+  uint32_t k;              /* -m : mer length, 1..128.  Keys are 1 (k <= 32), 2 (k <= 64) or 4 (k > 64) 64-bit
+                              words; k > 64 takes neither a Bloom structure (bf_size, bloom_counter) nor n_shards > 1,
+                              and is counted by direct insertion into the wide slot form (slot_bits 320)   */
   uint64_t size;           /* -s : requested number of table slots (GLOBAL table);
                               rounded up to 2^l and clipped to 4^k exactly like
                               large_hash::array (large_hash_array.hpp:992-1002)      */
@@ -112,7 +114,8 @@ typedef struct {
   uint32_t max_reprobe;    /* clipped limit (large_hash_array.hpp:29-39,160)           */
   uint32_t matrix_r, matrix_c;
   uint32_t matrix_identity;/* 1 when the table is as large as the key space            */
-  uint32_t slot_bits;      /* device slot width (32/64/128); informational            */
+  uint32_t slot_bits;      /* device slot width (32/64/128; 320 = the wide form of k > 64: a 64-bit head word
+                              [counter | ready | reprobe+1] and the 4-word key); informational */
   uint64_t local_slots;    /* slots resident on this device (incl. overflow margin)   */
   uint64_t table_bytes;
   const uint64_t* matrix_columns; /* matrix_c columns (NULL when identity); owned by
@@ -232,7 +235,7 @@ int  jfgpu_dump(jfgpu_handle h, uint64_t lower, uint64_t upper, uint32_t out_cou
                 jfgpu_sink_fn sink, void* ctx, uint64_t* n_records /* may be NULL */);
 
 /* -- lookup: array::get_val_for_key (large_hash_array.hpp:384-405).  keys: n packed
- *    k-mers in HOST memory (1 or 2 uint64 words each, word 0 first); vals: n counts
+ *    k-mers in HOST memory (1, 2 or 4 uint64 words each for k <= 32, <= 64, <= 128; word 0 first); vals: n counts
  *    (0 when absent).  Keys not owned by this shard give 0. */
 int  jfgpu_lookup(jfgpu_handle h, const uint64_t* keys, size_t n, uint64_t* vals);
 

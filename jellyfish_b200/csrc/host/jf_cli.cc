@@ -71,7 +71,9 @@ uint64_t parse_u64(const char* s, bool suffix, const char* name) {
   return v;
 }
 
-// 2-bit packed k-mer <-> text: first base in the most significant pair (mer_dna.hpp:451-462,525-542)
+// 2-bit packed k-mer <-> text: first base in the most significant pair (mer_dna.hpp:451-462,525-542).  A key is held in
+// MER_WORDS 64-bit words, word 0 least significant, whatever k (up to 128)
+constexpr unsigned MER_WORDS = 4;
 std::string mer_to_string(const uint64_t* w, unsigned k) {
   std::string s(k, 'A');
   for(unsigned i = 0; i < k; ++i) {
@@ -81,7 +83,7 @@ std::string mer_to_string(const uint64_t* w, unsigned k) {
   return s;
 }
 bool string_to_mer(const char* s, unsigned k, uint64_t* w) {
-  w[0] = w[1] = 0;
+  std::fill(w, w + MER_WORDS, 0);
   if(strlen(s) != k) return false;
   for(unsigned i = 0; i < k; ++i) {
     int c;
@@ -93,7 +95,7 @@ bool string_to_mer(const char* s, unsigned k, uint64_t* w) {
   return true;
 }
 void reverse_complement(const uint64_t* in, unsigned k, uint64_t* out) {
-  out[0] = out[1] = 0;
+  std::fill(out, out + MER_WORDS, 0);
   for(unsigned i = 0; i < k; ++i) {
     unsigned bit = 2 * i;
     uint64_t c = 3 - ((in[bit >> 6] >> (bit & 63)) & 3);
@@ -101,7 +103,11 @@ void reverse_complement(const uint64_t* in, unsigned k, uint64_t* out) {
     out[ob >> 6] |= c << (ob & 63);
   }
 }
-bool mer_less(const uint64_t* a, const uint64_t* b) { return a[1] != b[1] ? a[1] < b[1] : a[0] < b[0]; }
+bool mer_less(const uint64_t* a, const uint64_t* b) {
+  for(int q = MER_WORDS - 1; q > 0; --q) if(a[q] != b[q]) return a[q] < b[q];
+  return a[0] < b[0];
+}
+bool mer_equal(const uint64_t* a, const uint64_t* b) { return std::equal(a, a + MER_WORDS, b); }
 
 // ------------------------------------------------------------------------------------------
 // reader of the binary/sorted format (binary_dumper.hpp:83-109)
@@ -136,7 +142,7 @@ struct db_reader {
     if(header.format() == "binary/sorted") n_records = rec ? (file_size - body_off) / rec : 0;
   }
   void key_at(size_t i, uint64_t* w) const {
-    w[0] = w[1] = 0;
+    std::fill(w, w + MER_WORDS, 0);
     memcpy(w, base + body_off + i * rec, key_bytes);
   }
   uint64_t val_at(size_t i) const {
@@ -183,7 +189,7 @@ int file_sink(void* ctx, const void* recs, size_t n) {
   const unsigned char* p = (const unsigned char*)recs;
   std::string line;
   for(size_t off = 0; off + c->rec <= n; off += c->rec) {
-    uint64_t w[2] = {0, 0}, v = 0;
+    uint64_t w[MER_WORDS] = {0, 0, 0, 0}, v = 0;
     memcpy(w, p + off, c->key_bytes);
     memcpy(&v, p + off + c->key_bytes, 8);
     line = mer_to_string(w, c->k);
@@ -297,7 +303,7 @@ int bc_main(int argc, char* argv[]) {
   for(int i = optind; i < argc; ++i) files.push_back(argv[i]);
   if(!mer_given) usage_error("Missing required switch --mer-len");
   if(!size_given) usage_error("Missing required switch --size");
-  if(mer_len < 1 || mer_len > 64) usage_error("jellyfish-b200 supports mer lengths 1..64");
+  if(mer_len < 1 || mer_len > 64) usage_error("jellyfish-b200 bc supports mer lengths 1..64 (no Bloom counter for longer k-mers)");
   jfgpu_params p;
   memset(&p, 0, sizeof(p));
   p.struct_size = sizeof(p);
@@ -423,7 +429,8 @@ int count_main(int argc, char* argv[]) {
   }
   a.qual_given = a.min_qual != 0;
   if(a.disk && a.text) usage_error("--disk with --text is not supported by jellyfish-b200 (intermediate files are binary)");
-  if(a.mer_len < 1 || a.mer_len > 64) usage_error("jellyfish-b200 supports mer lengths 1..64");
+  if(a.mer_len < 1 || a.mer_len > 128) usage_error("jellyfish-b200 supports mer lengths 1..128");
+  if(a.mer_len > 64 && (a.bf_size_given || a.bc_given)) usage_error("--bf-size and --bc take mer lengths up to 64");
 
   header.canonical(a.canonical);
   jfgpu_params p;
@@ -544,7 +551,7 @@ int dump_main(int argc, char* argv[]) {
   if(db.header.format() != "binary/sorted") die("Unknown format '" + db.header.format() + "'");
   FILE* out = output ? fopen(output, "w") : stdout;
   if(!out) die(std::string("Error opening output file '") + output + "'");
-  uint64_t w[2];
+  uint64_t w[MER_WORDS];
   for(size_t i = 0; i < db.n_records; ++i) {
     uint64_t v = db.val_at(i);
     if(v < lower || v > upper) continue;
@@ -564,7 +571,7 @@ int dump_main(int argc, char* argv[]) {
 uint64_t db_lookup(const db_reader& db, const uint64_t* key) {
   const uint64_t pos = db.pos_of(key);
   size_t lo = 0, hi = db.n_records;
-  uint64_t w[2];
+  uint64_t w[MER_WORDS];
   while(lo < hi) {
     size_t mid = lo + (hi - lo) / 2;
     db.key_at(mid, w);
@@ -572,7 +579,7 @@ uint64_t db_lookup(const db_reader& db, const uint64_t* key) {
     bool less = mp != pos ? mp < pos : mer_less(w, key);
     if(less) lo = mid + 1; else hi = mid;
   }
-  if(lo < db.n_records) { db.key_at(lo, w); if(w[0] == key[0] && w[1] == key[1]) return db.val_at(lo); }
+  if(lo < db.n_records) { db.key_at(lo, w); if(mer_equal(w, key)) return db.val_at(lo); }
   return 0;
 }
 
@@ -624,7 +631,7 @@ int query_main(int argc, char* argv[]) {
   if(!out) die(std::string("Error opening output file '") + output + "'");
   const bool canonical = db.header.canonical();
   auto query_one = [&](const char* s) {
-    uint64_t m[2], r[2];
+    uint64_t m[MER_WORDS], r[MER_WORDS];
     if(!string_to_mer(s, db.k, m)) { fprintf(stderr, "Invalid mer '%s'\n", s); return; }
     const uint64_t* q = m;
     if(canonical) { reverse_complement(m, db.k, r); if(mer_less(r, m)) q = r; }
@@ -638,7 +645,7 @@ int query_main(int argc, char* argv[]) {
     if(!is.good()) die(std::string("Can't open file '") + path + "'");
     std::string line, seq;
     auto flush = [&]() {
-      uint64_t m[2] = {0, 0}, r[2] = {0, 0}; unsigned filled = 0;
+      uint64_t m[MER_WORDS] = {0, 0, 0, 0}, r[MER_WORDS] = {0, 0, 0, 0}; unsigned filled = 0;
       const unsigned k = db.k;
       for(char ch : seq) {
         int code;
@@ -646,10 +653,13 @@ int query_main(int argc, char* argv[]) {
                      case 'G': case 'g': code = 2; break; case 'T': case 't': code = 3; break; default: code = -1; }
         if(code < 0) { filled = 0; continue; }
         // shift left m, shift right r
-        uint64_t carry = m[0] >> 62;
-        m[0] = (m[0] << 2) | (uint64_t)code; m[1] = (m[1] << 2) | carry;
-        unsigned top = 2 * k; if(top < 64) m[0] &= ((uint64_t)1 << top) - 1, m[1] = 0; else if(top < 128) m[1] &= ((uint64_t)1 << (top - 64)) - 1;
-        r[0] = (r[0] >> 2) | (r[1] << 62); r[1] >>= 2;
+        for(int q = MER_WORDS - 1; q > 0; --q) m[q] = (m[q] << 2) | (m[q - 1] >> 62);
+        m[0] = (m[0] << 2) | (uint64_t)code;
+        const unsigned top = 2 * k;
+        for(unsigned q = 0; q < MER_WORDS; ++q)
+          if(top <= 64 * q) m[q] = 0; else if(top < 64 * (q + 1)) m[q] &= ((uint64_t)1 << (top - 64 * q)) - 1;
+        for(unsigned q = 0; q + 1 < MER_WORDS; ++q) r[q] = (r[q] >> 2) | (r[q + 1] << 62);
+        r[MER_WORDS - 1] >>= 2;
         unsigned ob = 2 * (k - 1); r[ob >> 6] |= (uint64_t)(3 - code) << (ob & 63);
         if(++filled >= k) {
           const uint64_t* q = (canonical && mer_less(r, m)) ? r : m;
@@ -827,11 +837,10 @@ void merge_dbs(const std::vector<std::string>& inputs, const char* output, jfb::
   std::ofstream out(output, std::ios::binary);
   if(!out.good()) die(std::string("Can't open out file '") + output + "'");
   if(op != MERGE_JACCARD) oh.write(out);
-  struct item { uint64_t pos; uint64_t key[2]; uint64_t val; int src; };
+  struct item { uint64_t pos; uint64_t key[MER_WORDS]; uint64_t val; int src; };
   auto greater = [](const item& a, const item& b) {
     if(a.pos != b.pos) return a.pos > b.pos;
-    if(a.key[1] != b.key[1]) return a.key[1] > b.key[1];
-    return a.key[0] > b.key[0];
+    return mer_less(b.key, a.key);
   };
   std::priority_queue<item, std::vector<item>, decltype(greater)> heap(greater);
   // cursors: record index in a binary body; byte offset of the next "MER count" line in a text body (text_dumper.hpp:50-80)
@@ -869,7 +878,7 @@ void merge_dbs(const std::vector<std::string>& inputs, const char* output, jfb::
     item top = heap.top();
     uint64_t sum = 0, minc = std::numeric_limits<uint64_t>::max(), maxc = 0;
     int present = 0;
-    while(!heap.empty() && heap.top().key[0] == top.key[0] && heap.top().key[1] == top.key[1]) {
+    while(!heap.empty() && mer_equal(heap.top().key, top.key)) {
       const int i = heap.top().src;
       const uint64_t v = heap.top().val;
       heap.pop();

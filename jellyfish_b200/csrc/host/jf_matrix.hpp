@@ -27,7 +27,7 @@ class gf2_matrix {
 public:
   gf2_matrix() : r_(0), c_(0), identity_(true) { }
   gf2_matrix(unsigned r, unsigned c) : r_(r), c_(c), identity_(false), col_(c, 0) {
-    if(r == 0 || r > 64 || c == 0) throw std::out_of_range("Invalid matrix size");
+    if(r == 0 || r > 64 || c == 0 || c > 256) throw std::out_of_range("Invalid matrix size");
   }
   template<typename It>
   gf2_matrix(unsigned r, unsigned c, It raw) : r_(r), c_(c), identity_(false), col_(c, 0) {
@@ -86,10 +86,10 @@ public:
   gf2_matrix pseudo_inverse() const {
     if(identity_) return *this;
     const unsigned s = std::min(r_, c_);
-    struct eq { uint64_t lo; uint64_t hi[2]; uint64_t w; };      // coefficients on vl, on vh, on w
+    struct eq { uint64_t lo; uint64_t hi[4]; uint64_t w; };      // coefficients on vl, on vh (c - s < 256 bits), on w
     std::vector<eq> R(s);
     for(unsigned j = 0; j < s; ++j) {
-      eq q = { 0, { 0, 0 }, (uint64_t)1 << j };
+      eq q = { 0, { 0, 0, 0, 0 }, (uint64_t)1 << j };
       for(unsigned i = 0; i < c_; ++i) {
         const uint64_t bit = (col_[c_ - 1 - i] >> j) & 1;          // key bit i feeds column c-1-i
         if(i < s) q.lo |= bit << i;
@@ -103,7 +103,7 @@ public:
       if(q == s) throw std::domain_error("hash matrix has no pseudo-inverse");
       std::swap(R[p], R[q]);
       for(unsigned t = 0; t < s; ++t)
-        if(t != p && ((R[t].lo >> p) & 1)) { R[t].lo ^= R[p].lo; R[t].hi[0] ^= R[p].hi[0]; R[t].hi[1] ^= R[p].hi[1]; R[t].w ^= R[p].w; }
+        if(t != p && ((R[t].lo >> p) & 1)) { R[t].lo ^= R[p].lo; for(int h = 0; h < 4; ++h) R[t].hi[h] ^= R[p].hi[h]; R[t].w ^= R[p].w; }
     }
     // row p now reads  vl_p = hi . vh ^ w . (M v)
     gf2_matrix res(r_, c_);

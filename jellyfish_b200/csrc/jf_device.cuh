@@ -19,7 +19,8 @@
 namespace jfk {
 
 constexpr int HALO  = 256;          // bytes of the previous tile staged again in front of a tile
-constexpr int PRE   = 64;           // symbol slots kept in front of a window (>= k-1)
+constexpr int PRE   = 64;           // symbol slots kept in front of a window (>= k-1) for k <= 64
+constexpr int PRE_WIDE = 128;       // the same for four-word keys (k <= 128)
 
 enum { ST_H = 0, ST_S = 1, ST_L = 2 };   // inside header line / inside sequence line / at line start
 constexpr uint32_t SYM_BREAK = 4;        // symbols 0..3 = A,C,G,T ; 4 = window reset
@@ -31,7 +32,7 @@ enum { STAT_KMERS = 0, STAT_INSERTED, STAT_DISTINCT, STAT_REPROBES, STAT_OVERFLO
 struct Carry {               // parser state handed from one batch to the next (device resident)
   uint32_t state;            // ST_* after the last byte of the previous batch
   uint32_t pad;
-  uint8_t  sym[PRE];         // last PRE symbols emitted (left-padded with SYM_BREAK)
+  uint8_t  sym[PRE_WIDE];    // last PRE (PRE_WIDE for four-word keys) symbols emitted (left-padded with SYM_BREAK)
 };
 
 struct TableDev {
@@ -480,10 +481,113 @@ __device__ __forceinline__ void table_add_batch(const TableDev& T, const uint64_
   }
 }
 
+// ---------------------------------------------------------------------------------------
+// The wide slot form (SB_WIDE, four-word keys, k = 65..128).  A quotiented key field would be 2k - l bits, up to 255, so
+// a slot holds the whole canonical key instead: 40 bytes = a 64-bit HEAD word
+//     head = [counter (high 64 - fbits bits) | READY (bit rbits) | reprobe+1 (low rbits bits)],  0 = empty,
+// followed by the four key words.  The key sits next to its head (one slot = five consecutive words), so a probe that
+// finds a head with its own reprobe index reads the key from the same or the next 32-byte sector.
+//
+// Claim / publish.  An inserter CASes the head from 0 to "claimed, not ready, reprobe i" (reprobe+1 alone), stores the
+// four key words, __threadfence(), then sets READY and adds its count with ONE atomicAdd.  A prober that meets a head
+// with its own reprobe index but without READY spins on the head until READY shows, fences, then compares the full key.
+// No deadlock: the only thread a waiter can wait on is the claimer of that slot, and between its CAS and its publishing
+// atomic the claimer executes four stores and a fence -- it waits on nothing and takes no other slot.  (Independent
+// thread scheduling, sm_70 and later, lets the claimer progress even when a waiter shares its warp.)  Ordering: the
+// claimer's fence + atomic is a release pattern, the waiter's load of READY + fence an acquire pattern, so the key words
+// are visible to it.  A head with another reprobe index belongs to another key (the same key always lands at the same
+// probe index from the same base) and is skipped without reading the key.
+// ---------------------------------------------------------------------------------------
+constexpr int SB_WIDE = 320;
+
+__device__ __forceinline__ unsigned long long* wide_slot(const TableDev& T, uint64_t idx) {
+  return (unsigned long long*)T.slots + 5 * idx;
+}
+__device__ __forceinline__ uint64_t ld_relaxed_u64(const unsigned long long* p) {
+  uint64_t v;
+  asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+// the head of a slot whose reprobe index is ours, once its key is published
+__device__ __forceinline__ uint64_t wide_wait_ready(const unsigned long long* s, uint64_t head, uint64_t ready) {
+  while(!(head & ready)) head = ld_relaxed_u64(s);
+  __threadfence();
+  return head;
+}
+__device__ __forceinline__ bool wide_key_eq(const unsigned long long* s, const uint64_t (&key)[4]) {
+  return ld_relaxed_u64(s + 1) == key[0] && ld_relaxed_u64(s + 2) == key[1] && ld_relaxed_u64(s + 3) == key[2] &&
+         ld_relaxed_u64(s + 4) == key[3];
+}
+// add c_lo << fbits to the head of an occupied slot; a carry out of the counter field and c_hi go to the side table
+__device__ __forceinline__ void wide_count(const TableDev& T, uint64_t idx, unsigned long long* s, uint64_t c_lo, uint64_t c_hi) {
+  const uint32_t fb = T.fbits, cb = 64 - fb;
+  uint64_t carry = c_hi;
+  if(c_lo) {
+    const uint64_t oc = (uint64_t)atomicAdd(s, (unsigned long long)(c_lo << fb)) >> fb;
+    if((oc + c_lo) >> cb) carry += 1;
+  }
+  if(carry) ovf_add(T, idx, carry);
+}
+
+// array::add / set / update_add (large_hash_array.hpp:291-347) on the wide form: T.op as in table_add_hp
+__device__ __forceinline__ bool wide_add(const TableDev& T, const uint64_t base, const uint64_t (&key)[4], uint64_t count, LocalStats& ls) {
+  const uint32_t rb = T.rbits, fb = T.fbits, cb = 64 - fb;
+  const uint64_t ready = 1ull << rb, rmask = ready - 1;
+  if(T.op == 1) count = 0;                   // PRIME: claim the key, add nothing
+  const uint64_t c_lo = count & ((1ull << cb) - 1), c_hi = count >> cb;
+  uint64_t idx = base;
+  for(uint32_t i = 0; i <= T.max_reprobe; ++i) {
+    unsigned long long* s = wide_slot(T, idx);
+    uint64_t head;
+    if(T.op == 2) {                          // UPDATE: never claims; an empty slot ends the probe sequence
+      head = ld_relaxed_u64(s);
+      if(head == 0) return true;
+    } else {
+      head = atomicCAS(s, 0ull, (unsigned long long)(i + 1));
+      if(head == 0) {
+        s[1] = key[0]; s[2] = key[1]; s[3] = key[2]; s[4] = key[3];
+        __threadfence();
+        atomicAdd(s, (unsigned long long)(ready | (c_lo << fb)));
+        if(c_hi) ovf_add(T, idx, c_hi);
+        ls.distinct++; ls.reprobes += i;
+        return true;
+      }
+    }
+    if((head & rmask) == i + 1) {
+      head = wide_wait_ready(s, head, ready);
+      if(wide_key_eq(s, key)) {
+        wide_count(T, idx, s, c_lo, c_hi);
+        ls.reprobes += i;
+        return true;
+      }
+    }
+    idx = base + tri(i + 1);
+  }
+  return T.op == 2;                          // (an update of an absent key is not a failure)
+}
+
+// count of `key` in the wide form (array::get_val_for_key), without the carries; false when absent
+__device__ __forceinline__ bool wide_find(const TableDev& T, const uint64_t base, const uint64_t (&key)[4], uint64_t& idx_out, uint64_t& cnt) {
+  const uint64_t rmask = (1ull << T.rbits) - 1;
+  uint64_t idx = base;
+  for(uint32_t i = 0; i <= T.max_reprobe; ++i) {
+    const unsigned long long* s = wide_slot(T, idx);
+    const uint64_t head = s[0];
+    if(head == 0) return false;
+    if((head & rmask) == i + 1 && s[1] == key[0] && s[2] == key[1] && s[3] == key[2] && s[4] == key[3]) {
+      idx_out = idx; cnt = head >> T.fbits;
+      return true;
+    }
+    idx = base + tri(i + 1);
+  }
+  return false;
+}
+
 template<int KW, int SB>
 __device__ __forceinline__ bool table_add(const TableDev& T, const uint64_t (&key)[KW], uint64_t pos_global,
                                           uint64_t count, LocalStats& ls) {
-  return table_add_hp<SB>(T, pos_global & T.local_mask, key_high<KW>(key, T.lsize), count, ls);
+  if constexpr(SB == SB_WIDE) return wide_add(T, pos_global & T.local_mask, key, count, ls);
+  else return table_add_hp<SB>(T, pos_global & T.local_mask, key_high<KW>(key, T.lsize), count, ls);
 }
 
 template<int KW>
@@ -504,7 +608,14 @@ template<int SB>
 __device__ __forceinline__ bool slot_decode(const TableDev& T, uint64_t idx, u128& high, uint32_t& reprobe, uint64_t& count) {
   const uint32_t rb = T.rbits, fb = T.fbits;
   const uint64_t rmask = (1ull << rb) - 1ull;
-  if(SB == 32) {
+  if(SB == SB_WIDE) {        // (the key is read from the slot by the callers that need it)
+    const uint64_t v = ((const uint64_t*)T.slots)[5 * idx];
+    if(v == 0) return false;
+    reprobe = (uint32_t)(v & rmask) - 1;
+    high.lo = 0; high.hi = 0;
+    count = v >> fb;
+    return true;
+  } else if(SB == 32) {
     uint32_t v = ((const uint32_t*)T.slots)[idx];
     if(v == 0) return false;
     uint32_t kf = v & ((1u << fb) - 1u);
@@ -531,6 +642,12 @@ __device__ __forceinline__ bool slot_decode(const TableDev& T, uint64_t idx, u12
     count = v.hi >> fhi;
     return true;
   }
+}
+
+// width of the in-slot counter field
+template<int SB>
+__device__ __forceinline__ uint32_t slot_counter_bits(const TableDev& T) {
+  return SB == SB_WIDE ? 64 - T.fbits : (SB == 128) ? (64 - (T.fbits > 64 ? T.fbits - 64 : 0)) : (SB - T.fbits);
 }
 
 }  // namespace jfk

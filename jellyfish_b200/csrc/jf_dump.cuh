@@ -41,7 +41,7 @@ struct DumpArgs {
 template<int SB>
 __device__ __forceinline__ uint64_t dump_full_count(const TableDev& T, uint64_t idx, uint64_t cnt, bool any_ovf) {
   if(!any_ovf) return cnt;
-  const uint32_t cb = (SB == 128) ? (64 - (T.fbits > 64 ? T.fbits - 64 : 0)) : (SB - T.fbits);
+  const uint32_t cb = slot_counter_bits<SB>(T);
   const uint64_t carries = ovf_get(T, idx);
   if(carries) {
     if(cb >= 64 || (carries >> (64 - cb)) != 0) return ~0ull;         // saturate like a 64-bit counter
@@ -165,6 +165,20 @@ __global__ void __launch_bounds__(DUMP_NTH) dump_emit_kernel(const DumpArgs a) {
       const uint32_t b = p ? cur[p - 1] : 0u, e = cur[p];
       for(uint32_t i = b + 1; i < e; ++i) {
         const uint16_t x = list[i];
+        if constexpr(SB == SB_WIDE) {            // four-word keys: compared from the most significant word down
+          const unsigned long long* sx = wide_slot(T, lo + x);
+          uint32_t j = i;
+          while(j > b) {
+            const unsigned long long* sy = wide_slot(T, lo + list[j - 1]);
+            int q = 3;
+            while(q > 0 && sy[1 + q] == sx[1 + q]) --q;
+            if(sy[1 + q] <= sx[1 + q]) break;
+            list[j] = list[j - 1];
+            --j;
+          }
+          list[j] = x;
+          continue;
+        }
         u128 hx; uint32_t rp; uint64_t c;
         slot_decode<SB>(T, lo + x, hx, rp, c);
         uint32_t j = i;
@@ -190,13 +204,20 @@ __global__ void __launch_bounds__(DUMP_NTH) dump_emit_kernel(const DumpArgs a) {
         cnt = dump_full_count<SB>(T, s, cnt, any_ovf);
         const uint64_t opos = s - (rp ? tri(rp) : 0);
         const uint64_t gpos = ((uint64_t)T.shard_index << T.local_lsize) | opos;
-        uint64_t v[KW], key[KW];
+        uint64_t key[KW];
+        if constexpr(SB == SB_WIDE) {
+          (void)gpos;
+#pragma unroll
+          for(int q = 0; q < KW; ++q) key[q] = wide_slot(T, s)[1 + q];
+        } else {
+        uint64_t v[KW];
         v[0] = (T.lsize >= 64 ? 0 : (high.lo << T.lsize)) | gpos;
         if(KW == 2) v[KW - 1] = T.lsize ? ((high.hi << T.lsize) | (high.lo >> (64 - T.lsize))) : high.hi;
         const uint64_t low = gf2_hash<KW>(lut, v, (int)a.nbytes);
 #pragma unroll
         for(int q = 0; q < KW; ++q) key[q] = v[q];
         key[0] = (key[0] & ~lmask) | (low & lmask);
+        }
         uint8_t* d = stage + threadIdx.x * rec;
         for(uint32_t b = 0; b < a.nbytes; ++b) d[b] = (uint8_t)(key[b >> 3] >> ((b & 7) * 8));
         if(cnt > maxv) cnt = maxv;

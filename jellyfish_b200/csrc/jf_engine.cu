@@ -18,6 +18,7 @@
 #include "jf_dump.cuh"
 #include "jf_shard.cuh"
 #include "jf_query.cuh"
+#include "jf_wide.cuh"
 
 using namespace jfk;
 
@@ -225,7 +226,10 @@ int table_setup(jfgpu_engine* e, Table& t, unsigned lsize, const jfb::gf2_matrix
   t.rbits = bitsize(limit + 1);
   t.fbits = t.hb + t.rbits;
   // at least 10 counter bits in a slot, so that only counts beyond ~1000 need the carry side table
-  if(t.fbits <= 22) t.slot_bits = 32;
+  if(e->kw == 4) {                 // four-word keys: the wide form, the whole key beside a head word (jf_device.cuh, SB_WIDE)
+    t.fbits = t.rbits + 1;         // the head's low bits: reprobe+1 and READY
+    t.slot_bits = SB_WIDE;
+  } else if(t.fbits <= 22) t.slot_bits = 32;
   else if(t.fbits <= 56) t.slot_bits = 64;
   else if(t.fbits <= 120) t.slot_bits = 128;
   else return fail(e, JFGPU_ERR_ARG, "key too long for this table size (key field > 120 bits)");
@@ -333,6 +337,38 @@ int dispatch(jfgpu_engine* e, unsigned kw, unsigned sb, F&& f) {
   return fail(e, JFGPU_ERR_ARG, "unsupported key/slot combination");
 }
 
+
+// The kernels of four-word keys, compiled in jf_wide.cu (jf_wide.cuh), with their types
+struct WideKernels {
+  void (*extract_count)(const CountArgs, const PartDev);
+  void (*extract_query)(const CountArgs, const PartDev);
+  void (*insert_keys)(TableDev, const uint64_t*, uint32_t, const uint64_t*, const uint64_t*, uint64_t);
+  void (*collect)(const CollectArgs);
+  void (*dump_count)(const DumpArgs);
+  void (*dump_emit)(const DumpArgs);
+  void (*lookup)(TableDev, const uint64_t*, uint32_t, const uint64_t*, uint64_t, uint64_t*, uint32_t);
+  void (*query_lookup)(TableDev, const uint64_t*, uint32_t, const uint64_t*, const uint32_t*, uint32_t, uint64_t, uint32_t, uint32_t,
+                       uint64_t*, unsigned long long*);
+  void (*query_decode)(const uint8_t*, uint64_t, uint32_t, uint32_t, uint64_t*, uint64_t*);
+  void (*query_format)(const uint64_t*, const uint64_t*, const uint32_t*, uint32_t, uint64_t, uint64_t, const unsigned long long*,
+                       uint32_t, uint8_t*);
+  void (*histogram)(TableDev, uint64_t, unsigned long long*, uint32_t);
+};
+template<typename F> void wide_cast(F& f, const void* p) { f = reinterpret_cast<F>(const_cast<void*>(p)); }
+const WideKernels& wide_kernels() {
+  static const WideKernels w = [] {
+    const jfw::Kernels& p = jfw::kernels();
+    WideKernels k;
+    wide_cast(k.extract_count, p.extract_count); wide_cast(k.extract_query, p.extract_query); wide_cast(k.insert_keys, p.insert_keys);
+    wide_cast(k.collect, p.collect); wide_cast(k.dump_count, p.dump_count); wide_cast(k.dump_emit, p.dump_emit);
+    wide_cast(k.lookup, p.lookup); wide_cast(k.query_lookup, p.query_lookup); wide_cast(k.query_decode, p.query_decode);
+    wide_cast(k.query_format, p.query_format); wide_cast(k.histogram, p.histogram);
+    return k;
+  }();
+  return w;
+}
+size_t wide_extract_smem(size_t lut_bytes) { return jfw::extract_smem(lut_bytes); }
+
 template<int NTH>
 size_t count_smem_bytes(size_t lut_bytes, size_t stage_bytes, size_t bloom_bytes = 0, bool fast = false) {
   const size_t part = fast ? (size_t)RING_P * 8 + (size_t)RING_P * RING * 4 : (stage_bytes ? PMAX * 4 + stage_bytes : 0);
@@ -400,6 +436,7 @@ void part_configure(jfgpu_engine* e) {
   PartState& ps = e->part;
   const Table& t = e->tab;
   ps.P = 0;
+  if(e->kw == 4) return;           // four-word keys: direct insertion only (no region records for the wide form)
   if(e->p.no_partition || t.bytes() < ((size_t)(e->p.part_min_mb ? e->p.part_min_mb : 256) << 20)) return;       // small tables live in L2 anyway
   uint32_t P = 256;
   const size_t region_target = (size_t)(e->p.region_mb ? e->p.region_mb : 64) << 20;
@@ -924,7 +961,12 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
     e->kev_used += 2;
     return JFGPU_OK;
   };
-  rc = dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int {
+  // four-word keys (jf_wide.cu): direct insertion (MODE 0) or query extraction (MODE 3) only
+  if(e->kw == 4) {
+    if(query) rc = launch(wide_kernels().extract_query, 512, wide_extract_smem(0), false);
+    else if(mode != 0 || part || shard_send || a.bloom.mode) rc = fail(e, JFGPU_ERR_ARG, "k > 64 is counted by direct insertion only (no sharding, no Bloom filter)");
+    else rc = launch(wide_kernels().extract_count, 512, wide_extract_smem(a.lut_bytes), false);
+  } else rc = dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int {
     constexpr int kw = decltype(KW)::value, sb = decltype(SB)::value;
     if(shard_send) {
       if(kw == 1 && e->tab.n_prow <= 2) return launch(extract_kernel<1, sb, 2, 1024, true, 2>, 1024, count_smem_bytes<1024>(a.lut_bytes, 0, 0, true), true);
@@ -1031,12 +1073,13 @@ int insert_keys_into(jfgpu_engine* e, Table& t, const uint64_t* keys, const uint
   TableDev T = table_dev(e, t);
   const size_t smem = (size_t)e->nbytes * 256 * 8;
   const int grid = (int)std::min<uint64_t>((n + 255) / 256, (uint64_t)e->n_sm * 8);
-  rc = dispatch(e, e->kw, t.slot_bits, [&](auto KW, auto SB) -> int {
-    auto kern = insert_keys_kernel<decltype(KW)::value, decltype(SB)::value>;
+  auto run = [&](auto kern) -> int {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     kern<<<grid, 256, smem, stream>>>(T, t.lut.as<uint64_t>(), e->nbytes, keys, counts, n);
     return JFGPU_OK;
-  });
+  };
+  rc = e->kw == 4 ? run(wide_kernels().insert_keys)
+                  : dispatch(e, e->kw, t.slot_bits, [&](auto KW, auto SB) -> int { return run(insert_keys_kernel<decltype(KW)::value, decltype(SB)::value>); });
   if(rc) return rc;
   JF_LAUNCHED();
   CUDA_OK(e, cudaGetLastError());
@@ -1078,12 +1121,13 @@ int collect_segment(jfgpu_engine* e, Table& t, SegScratch& s, uint64_t lo, uint6
   const size_t smem = (size_t)e->nbytes * 256 * 8;
   const uint64_t span = a.scan_hi - a.seg_lo;
   const int grid = (int)std::min<uint64_t>((span + 255) / 256, (uint64_t)e->n_sm * 16);
-  int rc = dispatch(e, e->kw, t.slot_bits, [&](auto KW, auto SB) -> int {
-    auto kern = collect_kernel<decltype(KW)::value, decltype(SB)::value>;
+  auto run = [&](auto kern) -> int {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     kern<<<grid, 256, smem, e->cs>>>(a);
     return JFGPU_OK;
-  });
+  };
+  int rc = e->kw == 4 ? run(wide_kernels().collect)
+                      : dispatch(e, e->kw, t.slot_bits, [&](auto KW, auto SB) -> int { return run(collect_kernel<decltype(KW)::value, decltype(SB)::value>); });
   if(rc) return rc;
   JF_LAUNCHED();
   unsigned long long n = 0;
@@ -1297,7 +1341,7 @@ int jfgpu_memcpy_h2d(void* dev_dst, const void* host_src, size_t bytes, void* st
 }
 
 int jfgpu_reference_matrix(uint32_t r, uint32_t c, uint32_t skip, uint64_t* cols) {
-  if(r == 0 || r > 64 || c == 0 || !cols) return JFGPU_ERR_ARG;
+  if(r == 0 || r > 64 || c == 0 || c > 256 || !cols) return JFGPU_ERR_ARG;
   jfb::glibc_random rng;
   jfb::gf2_matrix res;
   for(uint32_t i = 0; i <= skip; ++i) { jfb::gf2_matrix m(r, c); res = m.randomize_pseudo_inverse(rng); }
@@ -1308,12 +1352,15 @@ int jfgpu_reference_matrix(uint32_t r, uint32_t c, uint32_t skip, uint64_t* cols
 int jfgpu_create(const jfgpu_params* params, jfgpu_handle* out) {
   if(!params || !out) return fail(nullptr, JFGPU_ERR_ARG, "null argument");
   if(params->struct_size != sizeof(jfgpu_params)) return fail(nullptr, JFGPU_ERR_ARG, "jfgpu_params size mismatch");
-  if(params->k < 1 || params->k > 64) return fail(nullptr, JFGPU_ERR_ARG, "mer length must be in [1, 64]");
+  if(params->k < 1 || params->k > 128) return fail(nullptr, JFGPU_ERR_ARG, "mer length must be in [1, 128]");
   if(params->size == 0) return fail(nullptr, JFGPU_ERR_ARG, "size must be positive");
   uint32_t ns = params->n_shards ? params->n_shards : 1;
   if(ns & (ns - 1)) return fail(nullptr, JFGPU_ERR_ARG, "n_shards must be a power of two");
   if(params->shard_index >= ns) return fail(nullptr, JFGPU_ERR_ARG, "shard_index out of range");
   if(params->max_reprobe > 255) return fail(nullptr, JFGPU_ERR_ARG, "max_reprobe must be <= 255");
+  if(params->k > 64 && (params->bloom_counter || params->bf_size))
+    return fail(nullptr, JFGPU_ERR_ARG, "Bloom filters and counters take mer lengths up to 64");
+  if(params->k > 64 && ns > 1) return fail(nullptr, JFGPU_ERR_ARG, "sharded counting takes mer lengths up to 64");
 
   int ndev = 0;
   if(cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
@@ -1327,7 +1374,7 @@ int jfgpu_create(const jfgpu_params* params, jfgpu_handle* out) {
   e->p.n_shards = ns;
   e->device = params->device;
   e->k = params->k;
-  e->kw = params->k > 32 ? 2 : 1;
+  e->kw = params->k > 64 ? 4 : params->k > 32 ? 2 : 1;
   e->nbytes = (2 * params->k + 7) / 8;
   e->eff_val_len = params->counter_len;
   e->shard_bits = ceil_log2(ns);
@@ -1591,6 +1638,7 @@ int jfgpu_extract_route(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_
                         uint64_t* dev_counts, void* stream) {
   if(!e) return JFGPU_ERR_ARG;
   if(!e->tab.slots.p || e->bloom.mode != BLOOM_NONE) return fail(e, JFGPU_ERR_STATE, "Bloom filters are not supported on the sharded path");
+  if(e->kw == 4) return fail(e, JFGPU_ERR_ARG, "sharded counting takes mer lengths up to 64");
   if(((uintptr_t)dev_bytes & 15) != 0) return fail(e, JFGPU_ERR_ARG, "device text must be 16-byte aligned");
   cudaSetDevice(e->device);
   cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
@@ -1941,16 +1989,19 @@ int jfgpu_dump(jfgpu_handle e, uint64_t lower, uint64_t upper, uint32_t ocl, jfg
     a.n_tiles = (uint32_t)((a.seg_hi - a.seg_lo + DUMP_TP - 1) / DUMP_TP);
     a.tile_cnt = tile_cnt[b].as<uint32_t>(); a.out = out[b].as<uint8_t>(); a.out_cap = cap;
     const int grid = (int)std::min<uint64_t>(a.n_tiles, (uint64_t)e->n_sm * 8);
-    return dispatch(e, e->kw, t.slot_bits, [&](auto KW, auto SB) -> int {
-      constexpr int kw = decltype(KW)::value, sb = decltype(SB)::value;
-      dump_count_kernel<sb><<<grid, DUMP_NTH, 0, e->cs>>>(a); JF_LAUNCHED();
+    auto run = [&](auto count_kern, auto kern) -> int {
+      count_kern<<<grid, DUMP_NTH, 0, e->cs>>>(a); JF_LAUNCHED();
       dump_scan_kernel<<<1, 1024, 0, e->cs>>>(a.tile_cnt, a.n_tiles); JF_LAUNCHED();
-      auto kern = dump_emit_kernel<kw, sb>;
       cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       kern<<<grid, DUMP_NTH, smem, e->cs>>>(a); JF_LAUNCHED();
       CUDA_OK(e, cudaMemcpyAsync(h_total + b, a.tile_cnt + a.n_tiles, 4, cudaMemcpyDeviceToHost, e->cs));
       CUDA_OK(e, cudaEventRecord(ev_emit[b], e->cs));
       return JFGPU_OK;
+    };
+    if(e->kw == 4) return run(wide_kernels().dump_count, wide_kernels().dump_emit);
+    return dispatch(e, e->kw, t.slot_bits, [&](auto KW, auto SB) -> int {
+      constexpr int kw = decltype(KW)::value, sb = decltype(SB)::value;
+      return run(dump_count_kernel<sb>, dump_emit_kernel<kw, sb>);
     });
   };
   uint64_t n_in_buf[2] = { 0, 0 };
@@ -1996,12 +2047,13 @@ int jfgpu_lookup(jfgpu_handle e, const uint64_t* keys, size_t n, uint64_t* vals)
   TableDev T = table_dev(e, e->tab);
   const size_t smem = (size_t)e->nbytes * 256 * 8;
   const int grid = (int)std::min<uint64_t>((n + 255) / 256, (uint64_t)e->n_sm * 8);
-  int rc = dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int {
-    auto kern = lookup_kernel<decltype(KW)::value, decltype(SB)::value>;
+  auto run = [&](auto kern) -> int {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     kern<<<grid, 256, smem, e->cs>>>(T, e->tab.lut.as<uint64_t>(), e->nbytes, dk.as<uint64_t>(), n, dv.as<uint64_t>(), e->shard_bits);
     return JFGPU_OK;
-  });
+  };
+  int rc = e->kw == 4 ? run(wide_kernels().lookup)
+                      : dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int { return run(lookup_kernel<decltype(KW)::value, decltype(SB)::value>); });
   if(!rc) { JF_LAUNCHED();
     cudaError_t c = cudaMemcpyAsync(vals, dv.p, n * 8, cudaMemcpyDeviceToHost, e->cs);
     if(c == cudaSuccess) c = cudaStreamSynchronize(e->cs);
@@ -2050,6 +2102,7 @@ int jfgpu_load_records(jfgpu_handle e, const void* records, size_t nbytes, uint3
     if(c != cudaSuccess) { rc = fail(e, JFGPU_ERR_CUDA, std::string("load: ") + cudaGetErrorString(c)); break; }
     const int grid = (int)std::min<uint64_t>((m + 255) / 256, (uint64_t)e->n_sm * 8);
     if(e->kw == 1) query_decode_kernel<1><<<grid, 256, 0, e->cs>>>(raw.as<uint8_t>(), m, e->nbytes, counter_len, keys.as<uint64_t>(), counts.as<uint64_t>());
+    else if(e->kw == 4) wide_kernels().query_decode<<<grid, 256, 0, e->cs>>>(raw.as<uint8_t>(), m, e->nbytes, counter_len, keys.as<uint64_t>(), counts.as<uint64_t>());
     else query_decode_kernel<2><<<grid, 256, 0, e->cs>>>(raw.as<uint8_t>(), m, e->nbytes, counter_len, keys.as<uint64_t>(), counts.as<uint64_t>());
     JF_LAUNCHED();
     rc = insert_keys_into(e, e->tab, keys.as<uint64_t>(), counts.as<uint64_t>(), m, e->cs);
@@ -2113,13 +2166,14 @@ static int query_impl(jfgpu_engine* e, const char* bytes, size_t n, uint32_t fla
     e->stage_cur ^= 1;
     q.n_tiles = (len + TILE - 1) / TILE;
     const int grid = (int)std::min<uint64_t>(q.n_tiles, (uint64_t)e->n_sm * 8);
-    rc2 = dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int {
-      auto kern = query_lookup_kernel<decltype(KW)::value, decltype(SB)::value>;
+    auto run = [&](auto kern) -> int {
       cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lut_smem);
       kern<<<grid, QUERY_NTH, lut_smem, e->cs>>>(T, e->tab.lut.as<uint64_t>(), e->nbytes, q.keys.as<uint64_t>(), q.cnt.as<uint32_t>(), TILE,
                                                   q.n_tiles, e->k, 0, q.vals.as<uint64_t>(), q.off.as<unsigned long long>());
       return JFGPU_OK;
-    });
+    };
+    rc2 = e->kw == 4 ? run(wide_kernels().query_lookup)
+                     : dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int { return run(query_lookup_kernel<decltype(KW)::value, decltype(SB)::value>); });
     if(rc2) return rc2;
     JF_LAUNCHED();
     query_scan_kernel<<<1, 1024, 0, e->cs>>>(q.off.as<unsigned long long>(), q.n_tiles); JF_LAUNCHED();
@@ -2140,6 +2194,7 @@ static int query_impl(jfgpu_engine* e, const char* bytes, size_t n, uint32_t fla
     if(total) {
       const int grid = (int)std::min<uint64_t>(q.n_tiles, (uint64_t)e->n_sm * 8);
       if(e->kw == 1) query_format_kernel<1><<<grid, QUERY_NTH, 0, e->cs>>>(q.keys.as<uint64_t>(), q.vals.as<uint64_t>(), q.cnt.as<uint32_t>(), TILE, 0, q.n_tiles, q.off.as<unsigned long long>(), e->k, q.out.as<uint8_t>());
+      else if(e->kw == 4) wide_kernels().query_format<<<grid, QUERY_NTH, 0, e->cs>>>(q.keys.as<uint64_t>(), q.vals.as<uint64_t>(), q.cnt.as<uint32_t>(), TILE, 0, q.n_tiles, q.off.as<unsigned long long>(), e->k, q.out.as<uint8_t>());
       else query_format_kernel<2><<<grid, QUERY_NTH, 0, e->cs>>>(q.keys.as<uint64_t>(), q.vals.as<uint64_t>(), q.cnt.as<uint32_t>(), TILE, 0, q.n_tiles, q.off.as<unsigned long long>(), e->k, q.out.as<uint8_t>());
       JF_LAUNCHED();
       CUDA_OK(e, cudaGetLastError());
@@ -2217,6 +2272,7 @@ int jfgpu_histogram(jfgpu_handle e, uint64_t* hist, uint32_t n_bins) {
   switch(e->tab.slot_bits) {
   case 32:  histogram_kernel<32><<<grid, 256, 0, e->cs>>>(T, ns, dh.as<unsigned long long>(), n_bins); break;
   case 64:  histogram_kernel<64><<<grid, 256, 0, e->cs>>>(T, ns, dh.as<unsigned long long>(), n_bins); break;
+  case SB_WIDE: wide_kernels().histogram<<<grid, 256, 0, e->cs>>>(T, ns, dh.as<unsigned long long>(), n_bins); break;
   default:  histogram_kernel<128><<<grid, 256, 0, e->cs>>>(T, ns, dh.as<unsigned long long>(), n_bins); break;
   }
   JF_LAUNCHED();

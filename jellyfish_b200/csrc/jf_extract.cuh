@@ -22,12 +22,13 @@
 
 namespace jfk {
 
-template<int NTH>
+// PREN = symbol positions kept in front of the window: PRE, or PRE_WIDE for four-word keys
+template<int NTH, int PREN = PRE>
 struct __align__(16) ExtractSmemT {
   uint8_t  win[NTH * 32];            // TMA destination
-  uint32_t rev[2 * (NTH + 4)];       // 2-bit symbol stream, little endian: symbol s at bits 2(s&15) of rev[s>>4]
-  uint32_t brk[NTH + 4];             // reset stream: bit (s&31) of brk[s>>5]
-  uint8_t  pre[PRE];                 // byte symbols of the PRE stream positions in front of the window
+  uint32_t rev[2 * (NTH + PREN / 32 + 2)];   // 2-bit symbol stream, little endian: symbol s at bits 2(s&15) of rev[s>>4]
+  uint32_t brk[NTH + PREN / 32 + 2];         // reset stream: bit (s&31) of brk[s>>5]
+  uint8_t  pre[PREN];                // byte symbols of the PREN stream positions in front of the window
   uint64_t bar;
   uint32_t warp_fn[NTH / 32];
   uint32_t warp_cnt[NTH / 32];
@@ -117,11 +118,12 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
   constexpr int WINB = NTH * 32;
   constexpr int TILEB = WINB - HALO;
   constexpr int NW = NTH / 32;
-  constexpr int PW = PRE / 32;                   // 64-bit stream words in front of the window (PRE symbols)
+  constexpr int PREK = KW == 4 ? PRE_WIDE : PRE;  // symbol positions in front of the window (>= k - 1)
+  constexpr int PW = PREK / 32;                  // 64-bit stream words in front of the window (PREK symbols)
   constexpr int SG = 4;                          // k-mers whose shared-memory round trips are kept in flight together (FAST tail)
   extern __shared__ __align__(16) uint8_t smem_raw[];
-  ExtractSmemT<NTH>& sm = *reinterpret_cast<ExtractSmemT<NTH>*>(smem_raw);
-  uint64_t* lut = reinterpret_cast<uint64_t*>(smem_raw + ((sizeof(ExtractSmemT<NTH>) + 15) & ~(size_t)15));
+  ExtractSmemT<NTH, PREK>& sm = *reinterpret_cast<ExtractSmemT<NTH, PREK>*>(smem_raw);
+  uint64_t* lut = reinterpret_cast<uint64_t*>(smem_raw + ((sizeof(ExtractSmemT<NTH, PREK>) + 15) & ~(size_t)15));
   // per region: records in the open chunk (FAST: low 16 bits = records handed out, high 16 bits = records already written to
   // the chunk) and the open chunk's id; FAST: the rings behind them
   uint32_t* st_cnt = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(lut) + a.lut_bytes);
@@ -183,8 +185,8 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
       st_cnt[p] = cnt | (fl << 16);
     }
   };
-  for(uint32_t i = tid; i < 2 * (NTH + 4); i += NTH) sm.rev[i] = 0;
-  for(uint32_t i = tid; i < NTH + 4; i += NTH) sm.brk[i] = 0;
+  for(uint32_t i = tid; i < 2 * (NTH + PW + 2); i += NTH) sm.rev[i] = 0;
+  for(uint32_t i = tid; i < NTH + PW + 2; i += NTH) sm.brk[i] = 0;
   if(tid == 0) mbar_init(&sm.bar, 1);
   __syncthreads();
 
@@ -419,7 +421,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
     if(tid < HALO / 32 && bk) sm.halo_break = 1;
     if(cnt) {
       // OR the symbols into the packed streams at stream position PRE + off
-      const uint32_t pos = PRE + off;
+      const uint32_t pos = PREK + off;
       const uint32_t sh = (pos & 15u) * 2u;
       const uint32_t lo = (uint32_t)sy, hi = (uint32_t)(sy >> 32);
       const uint32_t x0 = lo << sh, x1 = __funnelshift_l(lo, hi, sh), x2 = __funnelshift_l(hi, 0u, sh);
@@ -443,23 +445,25 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
     if(warp == 0) {
       if(t == 0) {
         sm.pre[lane] = a.carry_in->sym[lane]; sm.pre[lane + 32] = a.carry_in->sym[lane + 32];
+        if constexpr(PREK > 64) { sm.pre[lane + 64] = a.carry_in->sym[lane + 64]; sm.pre[lane + 96] = a.carry_in->sym[lane + 96]; }
       } else {
         sm.pre[lane] = SYM_BREAK; sm.pre[lane + 32] = SYM_BREAK;
+        if constexpr(PREK > 64) { sm.pre[lane + 64] = SYM_BREAK; sm.pre[lane + 96] = SYM_BREAK; }
         __syncwarp();
         const bool in_seq = a.format == 1 ? (a.tile_state[t] == 1) : (a.tile_state[t] != ST_H);
         if(lane == 0 && in_seq && idx0 < k - 1 && !sm.halo_break) {
           // pathological input (very short lines / long runs of blank lines): exact slow path
-          if(a.format == 1) backfill_fastq(a.in, a.n_look, a.carry_in, h, PRE, sm.pre);
-          else backfill_symbols(a.in, a.n_look, a.carry_in, h, -2, PRE, sm.pre, a.min_qual != 0);
+          if(a.format == 1) backfill_fastq<PREK>(a.in, a.n_look, a.carry_in, h, PREK, sm.pre);
+          else backfill_symbols<PREK>(a.in, a.n_look, a.carry_in, h, -2, PREK, sm.pre, a.min_qual != 0);
         }
       }
       __syncwarp();
-      if(lane < PRE / 16) {                                 // one 32-bit word of 16 symbols per lane
+      if(lane < PREK / 16) {                                // one 32-bit word of 16 symbols per lane
         uint32_t x = 0;
         for(int i = 0; i < 16; ++i) x |= (uint32_t)(sm.pre[lane * 16 + i] & 3u) << (2 * i);
         sm.rev[lane] = x;
-      } else if(lane < PRE / 16 + PRE / 32) {
-        const int q = lane - PRE / 16;
+      } else if(lane < PREK / 16 + PREK / 32) {
+        const int q = lane - PREK / 16;
         uint32_t x = 0;
         for(int i = 0; i < 32; ++i) x |= (uint32_t)(sm.pre[q * 32 + i] >= SYM_BREAK) << i;
         sm.brk[q] = x;
@@ -471,16 +475,16 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
     if(t == a.n_tiles - 1 && warp == 1) {
       uint8_t* cs = a.carry_out->sym;
       const bool not_seq = a.format == 1 ? (a.tile_state[t] != 1) : (a.tile_state[t] == ST_H);
-      if(nsym >= (uint32_t)PRE || t == 0 || sm.halo_break || not_seq) {
+      if(nsym >= (uint32_t)PREK || t == 0 || sm.halo_break || not_seq) {
 #pragma unroll
-        for(int q = 0; q < 2; ++q) {                        // the last PRE symbols of the stream
+        for(int q = 0; q < PREK / 32; ++q) {                // the last PREK symbols of the stream
           const uint32_t s = nsym + lane + 32 * q;
           const uint32_t code = (sm.rev[s >> 4] >> (2 * (s & 15u))) & 3u;
           cs[lane + 32 * q] = (uint8_t)(((sm.brk[s >> 5] >> (s & 31u)) & 1u) ? SYM_BREAK : code);
         }
       } else if(lane == 0) {
-        if(a.format == 1) backfill_fastq(a.in, a.n_look, a.carry_in, (long long)n, PRE, cs);
-        else backfill_symbols(a.in, a.n_look, a.carry_in, (long long)n, -2, PRE, cs, a.min_qual != 0);
+        if(a.format == 1) backfill_fastq<PREK>(a.in, a.n_look, a.carry_in, (long long)n, PREK, cs);
+        else backfill_symbols<PREK>(a.in, a.n_look, a.carry_in, (long long)n, -2, PREK, cs, a.min_qual != 0);
       }
       if(lane == 0) a.carry_out->state = a.format == 1 ? (sm.total_state | (a.in[n - 1] == '\n' ? 4u : 0u)) : sm.total_state;
     }
@@ -492,7 +496,21 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
       const uint32_t W = PW + c;
       const int lo_i = (int)idx0 - (int)(32 * c), hi_i = (int)nsym - (int)(32 * c);
       uint32_t vmask = low_mask32((uint32_t)(hi_i > 32 ? 32 : hi_i)) & ~low_mask32((uint32_t)(lo_i < 0 ? 0 : (lo_i > 32 ? 32 : lo_i)));
-      {
+      if constexpr(KW == 4) {
+        // k > 32: a reset inside the word kills every end position from it on; of the resets in the 128 positions in front
+        // of the word only the last one matters, and it kills the end positions up to k - 1 past it
+        const uint32_t b0 = sm.brk[W];
+        if(b0) vmask &= low_mask32(__ffs(b0) - 1);
+#pragma unroll
+        for(int d = 1; d <= 4; ++d) {
+          const uint32_t bd = sm.brk[W - d];
+          if(bd) {
+            const int last = (31 - __clz(bd)) - 32 * d;              // relative to the word's first position (< 0)
+            if(last + (int)k > 0) vmask &= ~low_mask32((uint32_t)min(last + (int)k, 32));
+            break;
+          }
+        }
+      } else {
         // resets in the 96 symbols ending with this word (k <= 64): dilate by k-1 positions
         uint64_t b_lo = ((uint64_t)sm.brk[W] << 32) | sm.brk[W - 1];           // positions 32(W-1) .. 32W+31
         uint32_t b_pp = KW == 2 ? sm.brk[W - 2] : 0u;
@@ -540,6 +558,51 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
       q_rank = wo + qinc - pc;
       if(tid == NTH - 1) a.q_cnt[t] = q_rank + pc;
     }
+    if constexpr(KW == 4) {
+      // four-word keys (k = 65..128): MODE 0 (direct insertion) and MODE 3 (query extraction), one k-mer at a time.
+      // Key word q holds bases k-1-32q-31 .. k-1-32q from the end; the forward k-mer ending at stream position e is the
+      // pair reversal of the 32-symbol pieces ending at e, e-32, ...; its reverse complement is the complement of the
+      // pieces starting at e-k+1, e-k+33, ... (symbol s sits at bits 2(s&31) of rev64[s>>5])
+      auto piece = [&](const uint32_t s) -> uint64_t {        // the 32 symbols from stream position s on
+        const uint32_t w = s >> 5, sh = 2 * (s & 31u);
+        return sh ? ((rev64[w] >> sh) | (rev64[w + 1] << (64 - sh))) : rev64[w];
+      };
+      uint64_t kmask[4];
+#pragma unroll
+      for(int q = 0; q < 4; ++q) kmask[q] = kbits >= 64u * (q + 1) ? ~0ull : (kbits <= 64u * q ? 0ull : ((1ull << (kbits - 64 * q)) - 1ull));
+      for(uint32_t c = tid; c < n_words; c += NTH) {
+        const uint32_t vmask = kmer_mask(c);
+        if(!vmask) continue;
+        ls.kmers += __popc(vmask);
+        for(uint32_t r = vmask; r; r &= r - 1) {
+          const uint32_t j = __ffs(r) - 1;
+          const uint32_t e = 32 * (PW + c) + j;              // stream position of the k-mer's last base
+          uint64_t m[4], rc[4], key[4];
+#pragma unroll
+          for(int q = 0; q < 4; ++q) {
+            m[q] = pair_reverse64(piece(e - 32 * q - 31)) & kmask[q];
+            rc[q] = ~piece(e - k + 1 + 32 * q) & kmask[q];
+          }
+          bool use_rc = false;
+          if(a.canonical) {
+            int q = 3;
+            while(q > 0 && rc[q] == m[q]) --q;
+            use_rc = rc[q] < m[q];
+          }
+#pragma unroll
+          for(int q = 0; q < 4; ++q) key[q] = use_rc ? rc[q] : m[q];
+          if constexpr(MODE == 3) {
+            const uint64_t at = (uint64_t)t * a.q_tile_cap + q_rank + __popc(vmask & low_mask32(j));
+#pragma unroll
+            for(int q = 0; q < 4; ++q) a.q_keys[at * 4 + q] = key[q];
+          } else {
+            const uint64_t pos = gf2_hash<4>(lut, key, (int)a.nbytes);
+            if(table_add<4, SB>(a.T, key, pos, 1, ls)) ls.inserted++;
+            else { ls.failed++; record_failure<4>(a.T, key, 1); }
+          }
+        }
+      }
+    } else {
     // (FAST: every thread makes exactly one trip, with an empty mask if it owns no word -- the ring passes below are block-wide)
     for(uint32_t c = tid; c < (FAST ? (uint32_t)NTH : n_words); c += NTH) {
       const uint32_t W = PW + c;
@@ -701,6 +764,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
         }
         }
       }
+    }
     }
     __syncthreads();     // all reads of the streams done
     // clear the stream words this window used (the next window ORs into them) and roll full chunks over

@@ -237,6 +237,7 @@ __global__ void __launch_bounds__(256) bloom_unpack_kernel(const uint8_t* __rest
 // out[need-1-j] receives the j-th newest symbol, so out[0..need) ends up oldest-first;
 // missing leading entries are SYM_BREAK.  `line_nl` = position of the last '\n' before `end`
 // if known (>= -1), or -2 when unknown.
+template<int CPRE = PRE>               // symbols a Carry holds for this key width
 __device__ void backfill_symbols(const uint8_t* in, uint64_t n, const Carry* cin, long long end, long long line_nl,
                                  int need, uint8_t* out, bool keep_cr = false) {
   for(int i = 0; i < need; ++i) out[i] = SYM_BREAK;
@@ -270,7 +271,7 @@ __device__ void backfill_symbols(const uint8_t* in, uint64_t n, const Carry* cin
       if(got >= need) return;
     }
     if(q < 0) {                      // reached the batch start: continue into the previous batch's carry
-      for(int j = PRE - 1; j >= 0 && got < need; --j) {
+      for(int j = CPRE - 1; j >= 0 && got < need; --j) {
         uint32_t sy = cin->sym[j];
         if(sy == SYM_BREAK) return;
         out[need - 1 - got] = (uint8_t)sy; ++got;
@@ -284,13 +285,14 @@ __device__ void backfill_symbols(const uint8_t* in, uint64_t n, const Carry* cin
 // FASTQ slow path: a sequence line is never continued from another line, so the symbols before
 // `end` are those of the same line (back to its '\n'), then a reset; before the batch start the
 // previous batch's carry continues the line.
+template<int CPRE = PRE>
 __device__ void backfill_fastq(const uint8_t* in, uint64_t n, const Carry* cin, long long end, int need, uint8_t* out) {
   for(int i = 0; i < need; ++i) out[i] = SYM_BREAK;
   int got = 0;
   for(long long p = end - 1; got < need; --p) {
     if(p < 0) {
       if((cin->state & 3u) != 1u || (cin->state & 4u)) return;       // the batch did not start inside a sequence line
-      for(int j = PRE - 1; j >= 0 && got < need; --j) {
+      for(int j = CPRE - 1; j >= 0 && got < need; --j) {
         const uint32_t sy = cin->sym[j];
         if(sy == SYM_BREAK) return;
         out[need - 1 - got] = (uint8_t)sy; ++got;
@@ -918,7 +920,7 @@ __global__ void __launch_bounds__(256) collect_kernel(const CollectArgs a) {
       opos = idx - (rp ? tri(rp) : 0);
       if(opos >= a.seg_lo && opos < a.seg_hi) {
         if(T.stats[STAT_OVERFLOWED]) {
-          const uint32_t cb = (SB == 128) ? (64 - (T.fbits > 64 ? T.fbits - 64 : 0)) : (SB - T.fbits);
+          const uint32_t cb = slot_counter_bits<SB>(T);
           const uint64_t carries = ovf_get(T, idx);
           if(carries) {
             // saturate at 2^64-1 like a 64-bit counter would
@@ -936,7 +938,15 @@ __global__ void __launch_bounds__(256) collect_kernel(const CollectArgs a) {
       basei = __shfl_sync(0xffffffffu, basei, 0);
       if(have) {
         const uint64_t o = basei + __popc(ballot & ((1u << lane) - 1u));
-        if(o < a.out_cap) {
+        if constexpr(SB == SB_WIDE) {         // the key is in the slot; the records are only re-inserted (regrow)
+          if(o < a.out_cap) {
+            const unsigned long long* sl = wide_slot(T, idx);
+#pragma unroll
+            for(int q = 0; q < 4; ++q) a.out_keys[o * 4 + q] = sl[1 + q];
+            a.out_counts[o] = cnt;
+            a.out_sort_lo[o] = opos - a.seg_lo;
+          }
+        } else if(o < a.out_cap) {
           // global position = shard bits : local original position
           const uint64_t gpos = ((uint64_t)T.shard_index << T.local_lsize) | opos;
           // vector fed to the inverse matrix: [high bits of key : position]
@@ -980,6 +990,17 @@ template<int KW, int SB>
 __device__ __forceinline__ uint64_t table_get(const TableDev& T, const uint64_t (&key)[KW], uint64_t pos, uint32_t shard_bits) {
   const uint32_t owner = shard_bits ? (uint32_t)(pos >> (T.lsize - shard_bits)) : 0u;
   if(owner != T.shard_index) return 0;
+  if constexpr(SB == SB_WIDE) {
+    uint64_t idx = 0, cnt = 0;
+    if(!wide_find(T, pos & T.local_mask, key, idx, cnt)) return 0;
+    const uint32_t cb = slot_counter_bits<SB>(T);
+    const uint64_t carries = T.stats[STAT_OVERFLOWED] ? ovf_get(T, idx) : 0;
+    if(carries) {
+      if((carries >> (64 - cb)) != 0) cnt = ~0ull;
+      else { uint64_t add = carries << cb; cnt = (cnt + add < cnt) ? ~0ull : cnt + add; }
+    }
+    return cnt;
+  }
   const u128 want = key_high<KW>(key, T.lsize);
   const uint64_t base = pos & T.local_mask;
   uint64_t idx = base;
@@ -987,7 +1008,7 @@ __device__ __forceinline__ uint64_t table_get(const TableDev& T, const uint64_t 
     u128 high; uint32_t rp; uint64_t cnt;
     if(!slot_decode<SB>(T, idx, high, rp, cnt)) break;          // empty slot ends the probe sequence
     if(rp == r && high.lo == want.lo && high.hi == want.hi) {
-      const uint32_t cb = (SB == 128) ? (64 - (T.fbits > 64 ? T.fbits - 64 : 0)) : (SB - T.fbits);
+      const uint32_t cb = slot_counter_bits<SB>(T);
       const uint64_t carries = T.stats[STAT_OVERFLOWED] ? ovf_get(T, idx) : 0;
       if(carries) {
         if(cb >= 64 || (carries >> (64 - cb)) != 0) cnt = ~0ull;
@@ -1023,7 +1044,7 @@ __global__ void __launch_bounds__(256) histogram_kernel(TableDev T, uint64_t n_s
     u128 high; uint32_t rp; uint64_t cnt;
     if(slot_decode<SB>(T, idx, high, rp, cnt)) {
       if(T.stats[STAT_OVERFLOWED]) {
-        const uint32_t cb = (SB == 128) ? (64 - (T.fbits > 64 ? T.fbits - 64 : 0)) : (SB - T.fbits);
+        const uint32_t cb = slot_counter_bits<SB>(T);
         const uint64_t carries = ovf_get(T, idx);
         if(carries) {
           if(cb >= 64 || (carries >> (64 - cb)) != 0) cnt = ~0ull;
@@ -1042,7 +1063,7 @@ __global__ void __launch_bounds__(256) max_count_kernel(TableDev T, uint64_t n_s
     u128 high; uint32_t rp; uint64_t cnt;
     if(slot_decode<SB>(T, idx, high, rp, cnt)) {
       if(T.stats[STAT_OVERFLOWED]) {
-        const uint32_t cb = (SB == 128) ? (64 - (T.fbits > 64 ? T.fbits - 64 : 0)) : (SB - T.fbits);
+        const uint32_t cb = slot_counter_bits<SB>(T);
         const uint64_t carries = ovf_get(T, idx);
         if(carries) {
           if(cb >= 64 || (carries >> (64 - cb)) != 0) cnt = ~0ull;

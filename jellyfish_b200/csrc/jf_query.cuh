@@ -21,7 +21,7 @@ __global__ void __launch_bounds__(256) query_decode_kernel(const uint8_t* __rest
   const uint32_t rb = key_bytes + ocl;
   for(uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     const uint8_t* p = rec + i * rb;
-    uint64_t w[2] = { 0, 0 }, c = 0;
+    uint64_t w[KW > 2 ? 4 : 2] = { 0, 0 }, c = 0;
     for(uint32_t b = 0; b < key_bytes; ++b) w[b >> 3] |= (uint64_t)p[b] << (8 * (b & 7));
     for(uint32_t b = 0; b < ocl; ++b) c |= (uint64_t)p[key_bytes + b] << (8 * b);
 #pragma unroll

@@ -79,7 +79,7 @@ class HashCounter(object):
             raise JellyfishError(rc, self._lib.jfgpu_last_error(None).decode())
         self.k = k
         self.canonical = bool(canonical)
-        self.key_words = 2 if k > 32 else 1
+        self.key_words = 4 if k > 64 else 2 if k > 32 else 1       # 64-bit words per key (jfgpu_lookup)
         self.n_shards = n_shards
 
     # -- plumbing ---------------------------------------------------------------------------
@@ -220,9 +220,8 @@ class HashCounter(object):
             v = mer_to_int(m) if isinstance(m, str) else int(m)
             if self.canonical:
                 v = canonical_int(v, self.k)
-            keys[i * kw] = v & UINT64_MAX
-            if kw == 2:
-                keys[i * kw + 1] = v >> 64
+            for q in range(kw):
+                keys[i * kw + q] = (v >> (64 * q)) & UINT64_MAX
         vals = (C.c_uint64 * n)()
         self._check(self._lib.jfgpu_lookup(self._h, keys, n, vals))
         return list(vals)
