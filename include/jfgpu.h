@@ -52,8 +52,9 @@ enum { JFGPU_OP_COUNT = 0, JFGPU_OP_PRIME = 1, JFGPU_OP_UPDATE = 2 };
 typedef struct {
   uint32_t struct_size;    /* sizeof(jfgpu_params), for ABI evolution                */
   uint32_t k;              /* -m : mer length, 1..128.  Keys are 1 (k <= 32), 2 (k <= 64) or 4 (k > 64) 64-bit
-                              words; k > 64 takes neither a Bloom structure (bf_size, bloom_counter) nor n_shards > 1,
-                              and is counted by direct insertion into the wide slot form (slot_bits 320)   */
+                              words; k > 64 takes no Bloom structure (bf_size, bloom_counter) and at most 8 shards (the
+                              key exchange only: jfgpu_extract_route / jfgpu_insert_keys), and is counted by direct
+                              insertion into the wide slot form (slot_bits 320)   */
   uint64_t size;           /* -s : requested number of table slots (GLOBAL table);
                               rounded up to 2^l and clipped to 4^k exactly like
                               large_hash::array (large_hash_array.hpp:992-1002)      */
@@ -163,7 +164,8 @@ int  jfgpu_feed_device(jfgpu_handle h, const void* dev_bytes, size_t n, uint32_t
 /* -- multi-GPU stages (no reference analogue; SURVEY.md section 8e) ------------------
  * Extract canonical k-mers from device-resident text and bucket them by owning shard
  * (top bits of the hash position).  dev_keys: n_shards * capacity packed keys
- * (8 bytes each for k<=32, 16 for k<=64), bucket d at offset d*capacity;
+ * (8 bytes each for k<=32, 16 for k<=64, 32 for k<=128; word 0 first), bucket d at offset d*capacity;
+ * 16-byte aligned for k > 64;
  * dev_counts: n_shards uint64 counters (accumulated; caller zeroes).
  * Returns JFGPU_ERR_FULL if a bucket overflowed (counts still exact, keys truncated).
  * With a caller stream and neither FILE flag the call is stream-ordered (no host synchronisation;
@@ -172,7 +174,8 @@ int  jfgpu_extract_route(jfgpu_handle h, const void* dev_bytes, size_t n, uint32
                          void* dev_keys, uint64_t capacity, uint64_t* dev_counts, void* stream);
 /* Insert n packed keys (as produced by jfgpu_extract_route) that this shard owns:
  * hash_counter::add for each (hash_counter.hpp:91-115).  With a caller stream the call is
- * stream-ordered (returns without synchronising). */
+ * stream-ordered (returns without synchronising).  A shard's table never doubles: keys that find
+ * no slot are counted as failed and make jfgpu_finish return JFGPU_ERR_FULL ("Hash full"). */
 int  jfgpu_insert_keys(jfgpu_handle h, const void* dev_keys, uint64_t n, void* stream);
 
 /* Sharded counting, record exchange (the default for the geometries it covers -- k <= 21 with 32-bit slots; otherwise the

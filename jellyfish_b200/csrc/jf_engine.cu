@@ -353,6 +353,7 @@ struct WideKernels {
   void (*query_format)(const uint64_t*, const uint64_t*, const uint32_t*, uint32_t, uint64_t, uint64_t, const unsigned long long*,
                        uint32_t, uint8_t*);
   void (*histogram)(TableDev, uint64_t, unsigned long long*, uint32_t);
+  void (*extract_route)(const CountArgs, const PartDev);
 };
 template<typename F> void wide_cast(F& f, const void* p) { f = reinterpret_cast<F>(const_cast<void*>(p)); }
 const WideKernels& wide_kernels() {
@@ -362,7 +363,7 @@ const WideKernels& wide_kernels() {
     wide_cast(k.extract_count, p.extract_count); wide_cast(k.extract_query, p.extract_query); wide_cast(k.insert_keys, p.insert_keys);
     wide_cast(k.collect, p.collect); wide_cast(k.dump_count, p.dump_count); wide_cast(k.dump_emit, p.dump_emit);
     wide_cast(k.lookup, p.lookup); wide_cast(k.query_lookup, p.query_lookup); wide_cast(k.query_decode, p.query_decode);
-    wide_cast(k.query_format, p.query_format); wide_cast(k.histogram, p.histogram);
+    wide_cast(k.query_format, p.query_format); wide_cast(k.histogram, p.histogram); wide_cast(k.extract_route, p.extract_route);
     return k;
   }();
   return w;
@@ -961,10 +962,11 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
     e->kev_used += 2;
     return JFGPU_OK;
   };
-  // four-word keys (jf_wide.cu): direct insertion (MODE 0) or query extraction (MODE 3) only
+  // four-word keys (jf_wide.cu): direct insertion (MODE 0), keys bucketed by owner (MODE 1) or query extraction (MODE 3)
   if(e->kw == 4) {
     if(query) rc = launch(wide_kernels().extract_query, 512, wide_extract_smem(0), false);
-    else if(mode != 0 || part || shard_send || a.bloom.mode) rc = fail(e, JFGPU_ERR_ARG, "k > 64 is counted by direct insertion only (no sharding, no Bloom filter)");
+    else if(part || shard_send || a.bloom.mode) rc = fail(e, JFGPU_ERR_ARG, "k > 64 takes neither region records, the record exchange nor a Bloom filter");
+    else if(mode == 1) rc = launch(wide_kernels().extract_route, 512, wide_extract_smem(a.lut_bytes), false);
     else rc = launch(wide_kernels().extract_count, 512, wide_extract_smem(a.lut_bytes), false);
   } else rc = dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int {
     constexpr int kw = decltype(KW)::value, sb = decltype(SB)::value;
@@ -1360,7 +1362,7 @@ int jfgpu_create(const jfgpu_params* params, jfgpu_handle* out) {
   if(params->max_reprobe > 255) return fail(nullptr, JFGPU_ERR_ARG, "max_reprobe must be <= 255");
   if(params->k > 64 && (params->bloom_counter || params->bf_size))
     return fail(nullptr, JFGPU_ERR_ARG, "Bloom filters and counters take mer lengths up to 64");
-  if(params->k > 64 && ns > 1) return fail(nullptr, JFGPU_ERR_ARG, "sharded counting takes mer lengths up to 64");
+  if(params->k > 64 && ns > 8) return fail(nullptr, JFGPU_ERR_ARG, "sharded counting of mer lengths over 64 takes at most 8 shards");
 
   int ndev = 0;
   if(cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
@@ -1638,8 +1640,8 @@ int jfgpu_extract_route(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_
                         uint64_t* dev_counts, void* stream) {
   if(!e) return JFGPU_ERR_ARG;
   if(!e->tab.slots.p || e->bloom.mode != BLOOM_NONE) return fail(e, JFGPU_ERR_STATE, "Bloom filters are not supported on the sharded path");
-  if(e->kw == 4) return fail(e, JFGPU_ERR_ARG, "sharded counting takes mer lengths up to 64");
   if(((uintptr_t)dev_bytes & 15) != 0) return fail(e, JFGPU_ERR_ARG, "device text must be 16-byte aligned");
+  if(e->kw == 4 && ((uintptr_t)dev_keys & 15) != 0) return fail(e, JFGPU_ERR_ARG, "route buckets of four-word keys must be 16-byte aligned");
   cudaSetDevice(e->device);
   cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
   int first = -1;
@@ -1678,6 +1680,7 @@ int jfgpu_shard_setup(jfgpu_handle e, const jfgpu_shard_buffers* b) {
   // geometry the record exchange covers: one key word, the 32-bit hash tail, 4-byte records of the GLOBAL regions, the
   // receiver's own partition in 4-byte records drained by the window kernels
   const Table& t = e->tab;
+  if(e->kw == 4) return fail(e, JFGPU_ERR_ARG, "the record exchange takes mer lengths up to 64 (k > 64 uses the key exchange)");
   if(G < 2 || G > 8 || !t.slots.p || e->kw != 1 || !t.hash_fast || t.n_prow > 6 || t.lsize > 38 || t.slot_bits != 32 || e->bloom.mode != BLOOM_NONE ||
      !e->part.P || e->part.rec_bytes != 4 || e->part.P > RING_P)
     return fail(e, JFGPU_ERR_ARG, "this table geometry is not covered by the record exchange (use the key exchange)");

@@ -559,7 +559,8 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
       if(tid == NTH - 1) a.q_cnt[t] = q_rank + pc;
     }
     if constexpr(KW == 4) {
-      // four-word keys (k = 65..128): MODE 0 (direct insertion) and MODE 3 (query extraction), one k-mer at a time.
+      // four-word keys (k = 65..128): MODE 0 (direct insertion), MODE 1 (keys bucketed by owning shard) and MODE 3 (query
+      // extraction), one k-mer at a time.
       // Key word q holds bases k-1-32q-31 .. k-1-32q from the end; the forward k-mer ending at stream position e is the
       // pair reversal of the 32-symbol pieces ending at e, e-32, ...; its reverse complement is the complement of the
       // pieces starting at e-k+1, e-k+33, ... (symbol s sits at bits 2(s&31) of rev64[s>>5])
@@ -595,6 +596,21 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
             const uint64_t at = (uint64_t)t * a.q_tile_cap + q_rank + __popc(vmask & low_mask32(j));
 #pragma unroll
             for(int q = 0; q < 4; ++q) a.q_keys[at * 4 + q] = key[q];
+          } else if constexpr(MODE == 1) {
+            // the owner's bucket, as for k <= 64: one atomic per group of lanes with the same owner, then 32 bytes per key
+            // in two 16-byte stores (the host checks that the buckets are 16-byte aligned)
+            const uint64_t pos = gf2_hash<4>(lut, key, (int)a.nbytes);
+            const uint32_t owner = a.shard_bits ? (uint32_t)(pos >> (a.T.lsize - a.shard_bits)) : 0u;
+            const uint32_t peers = __match_any_sync(__activemask(), owner);
+            const uint32_t leader = __ffs(peers) - 1;
+            unsigned long long at = 0;
+            if((uint32_t)lane == leader) at = atomicAdd(&a.route_counts[owner], (unsigned long long)__popc(peers));
+            at = __shfl_sync(peers, at, leader) + __popc(peers & ((1u << lane) - 1u));
+            if(at < a.route_cap) {
+              ulonglong2* dst = reinterpret_cast<ulonglong2*>(a.route_keys + ((uint64_t)owner * a.route_cap + at) * 4);
+              dst[0] = make_ulonglong2(key[0], key[1]);
+              dst[1] = make_ulonglong2(key[2], key[3]);
+            } else atomicAdd(&a.T.stats[STAT_ROUTE_DROPPED], 1ull);
           } else {
             const uint64_t pos = gf2_hash<4>(lut, key, (int)a.nbytes);
             if(table_add<4, SB>(a.T, key, pos, 1, ls)) ls.inserted++;

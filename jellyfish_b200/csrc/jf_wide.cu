@@ -25,6 +25,7 @@ const Kernels& kernels() {
     (const void*)query_decode_kernel<4>,
     (const void*)query_format_kernel<4>,
     (const void*)histogram_kernel<SB_WIDE>,
+    (const void*)extract_kernel<4, SB_WIDE, 1, 512, false>,
   };
   return k;
 }

@@ -22,6 +22,7 @@ struct Kernels {                   // host stubs of the kernels (the argument ty
   const void* query_decode;        // query_decode_kernel<4>
   const void* query_format;        // query_format_kernel<4>
   const void* histogram;           // histogram_kernel<SB_WIDE>
+  const void* extract_route;       // extract_kernel<4, SB_WIDE, 1, 512, false>: keys bucketed by owning shard
 };
 const Kernels& kernels();
 size_t extract_smem(size_t lut_bytes);    // dynamic shared memory of extract_kernel<4, ...> besides the hash tables

@@ -9,7 +9,7 @@ the positions whose top log2(world) bits equal r, so the rank-ordered concatenat
 shard dumps is byte-identical to the single-GPU dump.
 
 Two forms of the exchange: 4-byte region RECORDS (RecordExchange, the default where the table geometry allows it: k <= 21,
-32-bit slots) and packed KEYS (any geometry).  The exchange logic (bucket capacities, count exchange, uneven all-to-all,
+32-bit slots) and packed KEYS (any geometry: 8, 16 or 32 bytes a key for k <= 32, k <= 64 and k <= 128).  The exchange logic (bucket capacities, count exchange, uneven all-to-all,
 ordering of the shard files) is plain torch.distributed code and is exercised on CPU with the gloo backend in
 tests/test_distributed_cpu.py through the `RouteBackend` seam below.
 """
@@ -205,12 +205,22 @@ class RecordExchange(object):
         self.trace = {"rounds": rounds_all, "extract_ms": t[0], "exchange_ms": t[1], "restage_ms": t[2]}
 
 
+def default_batch_bytes(k):
+    """Text per exchange round of the key exchange.  Its three buffers (send, the second send bank, recv) take about
+    8 * key_words * 1.25 bytes per batch byte each: 256 MB batches for k <= 64 (one or two key words), 64 MB for four-word
+    keys (k > 64), whose 256 MB batches would take about 32 GB and leave no room for a wide shard of 2^30 slots (43 GB)
+    on an 80 GB card."""
+    return (64 << 20) if k is not None and k > 64 else (256 << 20)
+
+
 class ShardedCounter(object):
     """hash_counter over `world` GPUs.  `size` is the GLOBAL table size (jellyfish count -s)."""
 
     def __init__(self, size, val_len=7, k=None, canonical=False, rank=0, world=1, device=0, reprobes=126,
-                 batch_bytes=256 << 20, slack=1.25, exchange="auto", send_gb=None, **engine_kw):
+                 batch_bytes=None, slack=1.25, exchange="auto", send_gb=None, **engine_kw):
         from .engine import HashCounter
+        if batch_bytes is None:
+            batch_bytes = default_batch_bytes(k)
         self.rank, self.world = rank, world
         self.hc = HashCounter(size, val_len, k=k, canonical=canonical, reprobes=reprobes, device=device,
                               shard_index=rank, n_shards=world, allow_regrow=(world == 1), max_batch_bytes=batch_bytes, **engine_kw)
