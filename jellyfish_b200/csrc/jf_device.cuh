@@ -184,6 +184,27 @@ __device__ __forceinline__ u128 key_high(const uint64_t (&key)[KW], uint32_t lsi
   return r;
 }
 
+// global position of a slot of this shard: shard bits : local position
+__device__ __forceinline__ uint64_t global_pos(const TableDev& T, uint64_t local_pos) {
+  return ((uint64_t)T.shard_index << T.local_lsize) | local_pos;
+}
+
+// the inverse of key_high and the hash: the key whose explicit bits are `high` and whose hash is the global position
+// `gpos`.  The low lsize key bits are the inverse matrix times [high : gpos] (large_hash_iterator.hpp:164-170;
+// large_hash_array.hpp:851-858).
+template<int KW>
+__device__ __forceinline__ void key_from_position(const uint64_t* __restrict__ inv_lut, uint32_t nbytes, uint32_t lsize, u128 high,
+                                                  uint64_t gpos, uint64_t (&key)[KW]) {
+  uint64_t v[KW];
+  v[0] = (lsize >= 64 ? 0 : (high.lo << lsize)) | gpos;
+  if(KW == 2) v[KW - 1] = lsize ? ((high.hi << lsize) | (high.lo >> (64 - lsize))) : high.hi;
+  const uint64_t low = gf2_hash<KW>(inv_lut, v, (int)nbytes);
+  const uint64_t lmask = lsize >= 64 ? ~0ull : ((1ull << lsize) - 1ull);
+#pragma unroll
+  for(int q = 0; q < KW; ++q) key[q] = v[q];
+  key[0] = (key[0] & ~lmask) | (low & lmask);
+}
+
 // ---------------------------------------------------------------------------------------
 // Bloom filter / Bloom counter operations
 // ---------------------------------------------------------------------------------------
@@ -276,6 +297,22 @@ __device__ __forceinline__ uint64_t ovf_get(const TableDev& T, uint64_t slot_idx
 // no slot ("hash full").  SB = slot width in bits.
 // ---------------------------------------------------------------------------------------
 struct LocalStats { uint32_t kmers, inserted, distinct, reprobes, failed; };
+
+// the end of an inserting kernel: a warp's insertion statistics summed over the warp, one atomic per nonzero sum
+__device__ __forceinline__ void flush_stats(unsigned long long* stats, unsigned long long inserted, unsigned long long distinct,
+                                            unsigned long long reprobes) {
+  unsigned long long v[3] = { inserted, distinct, reprobes };
+#pragma unroll
+  for(int q = 0; q < 3; ++q) {
+#pragma unroll
+    for(int o = 16; o; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
+  }
+  if((threadIdx.x & 31) == 0) {
+    if(v[0]) atomicAdd(&stats[STAT_INSERTED], v[0]);
+    if(v[1]) atomicAdd(&stats[STAT_DISTINCT], v[1]);
+    if(v[2]) atomicAdd(&stats[STAT_REPROBES], v[2]);
+  }
+}
 
 template<int SB> __device__ __forceinline__ bool slot_decode(const TableDev& T, uint64_t idx, u128& high, uint32_t& reprobe, uint64_t& count);
 
@@ -648,6 +685,20 @@ __device__ __forceinline__ bool slot_decode(const TableDev& T, uint64_t idx, u12
 template<int SB>
 __device__ __forceinline__ uint32_t slot_counter_bits(const TableDev& T) {
   return SB == SB_WIDE ? 64 - T.fbits : (SB == 128) ? (64 - (T.fbits > 64 ? T.fbits - 64 : 0)) : (SB - T.fbits);
+}
+
+// the count of slot `idx` whose counter field holds `cnt`, with the carries of the side table; saturates at 2^64-1 like a
+// 64-bit counter would.  (The callers skip it while no counter has ever carried: STAT_OVERFLOWED == 0.)  Only a 128-bit
+// slot can have a 64-bit counter field; a wide slot's is at most 62 bits (fbits >= 2).
+template<int SB>
+__device__ __forceinline__ uint64_t slot_full_count(const TableDev& T, uint64_t idx, uint64_t cnt) {
+  const uint32_t cb = slot_counter_bits<SB>(T);
+  const uint64_t carries = ovf_get(T, idx);
+  if(carries) {
+    if((SB != SB_WIDE && cb >= 64) || (carries >> (64 - cb)) != 0) cnt = ~0ull;
+    else { const uint64_t add = carries << cb; cnt = (cnt + add < cnt) ? ~0ull : cnt + add; }
+  }
+  return cnt;
 }
 
 }  // namespace jfk

@@ -39,19 +39,6 @@ struct DumpArgs {
 };
 
 template<int SB>
-__device__ __forceinline__ uint64_t dump_full_count(const TableDev& T, uint64_t idx, uint64_t cnt, bool any_ovf) {
-  if(!any_ovf) return cnt;
-  const uint32_t cb = slot_counter_bits<SB>(T);
-  const uint64_t carries = ovf_get(T, idx);
-  if(carries) {
-    if(cb >= 64 || (carries >> (64 - cb)) != 0) return ~0ull;         // saturate like a 64-bit counter
-    const uint64_t add = carries << cb;
-    return (cnt + add < cnt) ? ~0ull : cnt + add;
-  }
-  return cnt;
-}
-
-template<int SB>
 __global__ void __launch_bounds__(DUMP_NTH) dump_count_kernel(const DumpArgs a) {
   const TableDev& T = a.T;
   const bool any_ovf = T.stats[STAT_OVERFLOWED] != 0;
@@ -66,7 +53,7 @@ __global__ void __launch_bounds__(DUMP_NTH) dump_count_kernel(const DumpArgs a) 
       if(!slot_decode<SB>(T, s, high, rp, cnt)) continue;
       const uint64_t opos = s - (rp ? tri(rp) : 0);
       if(opos < lo || opos >= hi) continue;
-      cnt = dump_full_count<SB>(T, s, cnt, any_ovf);
+      if(any_ovf) cnt = slot_full_count<SB>(T, s, cnt);
       if(cnt >= a.lower && cnt <= a.upper) ++n;
     }
 #pragma unroll
@@ -109,7 +96,6 @@ __global__ void __launch_bounds__(DUMP_NTH) dump_emit_kernel(const DumpArgs a) {
   const bool any_ovf = T.stats[STAT_OVERFLOWED] != 0;
   const uint32_t rec = a.nbytes + a.ocl;
   const uint64_t maxv = a.ocl >= 8 ? ~0ull : ((1ull << (8 * a.ocl)) - 1ull);
-  const uint64_t lmask = T.lsize >= 64 ? ~0ull : ((1ull << T.lsize) - 1ull);
   for(uint32_t i = threadIdx.x; i < a.nbytes * 256u; i += DUMP_NTH) lut[i] = a.inv_lut[i];
 
   for(uint32_t tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
@@ -127,7 +113,7 @@ __global__ void __launch_bounds__(DUMP_NTH) dump_emit_kernel(const DumpArgs a) {
       if(!slot_decode<SB>(T, s, high, rp, cnt)) continue;
       const uint64_t opos = s - (rp ? tri(rp) : 0);
       if(opos < lo || opos >= hi) continue;
-      cnt = dump_full_count<SB>(T, s, cnt, any_ovf);
+      if(any_ovf) cnt = slot_full_count<SB>(T, s, cnt);
       if(cnt >= a.lower && cnt <= a.upper) atomicAdd(&cur[opos - lo], 1u);
     }
     __syncthreads();
@@ -155,7 +141,7 @@ __global__ void __launch_bounds__(DUMP_NTH) dump_emit_kernel(const DumpArgs a) {
       if(!slot_decode<SB>(T, s, high, rp, cnt)) continue;
       const uint64_t opos = s - (rp ? tri(rp) : 0);
       if(opos < lo || opos >= hi) continue;
-      cnt = dump_full_count<SB>(T, s, cnt, any_ovf);
+      if(any_ovf) cnt = slot_full_count<SB>(T, s, cnt);
       if(cnt >= a.lower && cnt <= a.upper) list[atomicAdd(&cur[opos - lo], 1u)] = (uint16_t)(s - lo);
     }
     __syncthreads();
@@ -201,23 +187,13 @@ __global__ void __launch_bounds__(DUMP_NTH) dump_emit_kernel(const DumpArgs a) {
         const uint64_t s = lo + list[i];
         u128 high; uint32_t rp; uint64_t cnt;
         slot_decode<SB>(T, s, high, rp, cnt);
-        cnt = dump_full_count<SB>(T, s, cnt, any_ovf);
+        if(any_ovf) cnt = slot_full_count<SB>(T, s, cnt);
         const uint64_t opos = s - (rp ? tri(rp) : 0);
-        const uint64_t gpos = ((uint64_t)T.shard_index << T.local_lsize) | opos;
         uint64_t key[KW];
         if constexpr(SB == SB_WIDE) {
-          (void)gpos;
 #pragma unroll
           for(int q = 0; q < KW; ++q) key[q] = wide_slot(T, s)[1 + q];
-        } else {
-        uint64_t v[KW];
-        v[0] = (T.lsize >= 64 ? 0 : (high.lo << T.lsize)) | gpos;
-        if(KW == 2) v[KW - 1] = T.lsize ? ((high.hi << T.lsize) | (high.lo >> (64 - T.lsize))) : high.hi;
-        const uint64_t low = gf2_hash<KW>(lut, v, (int)a.nbytes);
-#pragma unroll
-        for(int q = 0; q < KW; ++q) key[q] = v[q];
-        key[0] = (key[0] & ~lmask) | (low & lmask);
-        }
+        } else key_from_position<KW>(lut, a.nbytes, T.lsize, high, global_pos(T, opos), key);
         uint8_t* d = stage + threadIdx.x * rec;
         for(uint32_t b = 0; b < a.nbytes; ++b) d[b] = (uint8_t)(key[b >> 3] >> ((b & 7) * 8));
         if(cnt > maxv) cnt = maxv;

@@ -147,10 +147,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
   if(MODE == 2) {
     for(uint32_t p = tid; p < pd.P; p += NTH) {
       uint32_t c = my_chunk[p], f = my_fill[p];
-      if(c == NO_CHUNK) {
-        c = alloc_chunk(pd, pd.by_owner ? (p >> pd.owner_shift) : blockIdx.x); f = 0;
-        if(c == NO_CHUNK) { atomicAdd(&a.T.stats[STAT_POOL_FULL], 1ull); f = pd.chunk_recs; }
-      }
+      if(c == NO_CHUNK) c = fresh_chunk(pd, pd.by_owner ? (p >> pd.owner_shift) : blockIdx.x, a.T.stats, f);
       st_chunk[p] = c; st_cnt[p] = FAST ? (f | (f << 16)) : f;
     }
   }
@@ -763,19 +760,10 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
             const uint64_t lpos = pos & a.T.local_mask;
             const uint32_t p = (uint32_t)(lpos >> pd.region_bits);
             const uint64_t rel = lpos & ((1ull << pd.region_bits) - 1ull);
-            const u128 high = key_high<KW>(key, a.T.lsize);
-            const uint32_t hb = a.T.fbits - a.T.rbits;
-            u128 rec;
-            if(hb == 0)       { rec.lo = rel; rec.hi = 0; }
-            else if(hb < 64)  { rec.lo = high.lo | (rel << hb); rec.hi = high.hi | (rel >> (64 - hb)); }
-            else              { rec.lo = high.lo; rec.hi = high.hi | (rel << (hb - 64)); }
+            const u128 rec = rec_make(key_high<KW>(key, a.T.lsize), rel, a.T.fbits - a.T.rbits);
             const uint32_t slot = atomicAdd(&st_cnt[p], 1u);
-            if(slot < pd.chunk_recs) {
-              uint8_t* dst = pd.pool + (size_t)st_chunk[p] * CHUNK_BYTES;
-              if(pd.rec_bytes == 4) reinterpret_cast<uint32_t*>(dst)[slot] = (uint32_t)rec.lo;
-              else if(pd.rec_bytes == 8) reinterpret_cast<uint64_t*>(dst)[slot] = rec.lo;
-              else { reinterpret_cast<uint64_t*>(dst)[2 * slot] = rec.lo; reinterpret_cast<uint64_t*>(dst)[2 * slot + 1] = rec.hi; }
-            } else spill_record<KW, SB>(a.T, pd.spill_keys, pd.spill_counts, pd.spill_n, pd.spill_cap, key[0], key[KW - 1], pos, pd.lazy_win);    // this region's chunk filled up within one window (skewed input)
+            if(slot < pd.chunk_recs) store_rec(pd.pool + (size_t)st_chunk[p] * CHUNK_BYTES, pd.rec_bytes, slot, rec);
+            else spill_record<KW, SB>(a.T, pd.spill_keys, pd.spill_counts, pd.spill_n, pd.spill_cap, key[0], key[KW - 1], pos, pd.lazy_win);    // this region's chunk filled up within one window (skewed input)
           }
         }
         }
@@ -786,18 +774,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
     // clear the stream words this window used (the next window ORs into them) and roll full chunks over
     for(uint32_t i = tid; i < 2 * (n_words + PW) + 3; i += NTH) sm.rev[i] = 0;
     for(uint32_t i = tid; i < n_words + PW + 2; i += NTH) sm.brk[i] = 0;
-    if(MODE == 2 && !FAST) {
-      for(uint32_t p = tid; p < pd.P; p += NTH) {
-        const uint32_t c = st_cnt[p];
-        if(c + pd.margin > pd.chunk_recs) {
-          const uint32_t old = st_chunk[p];
-          if(old != NO_CHUNK) pd.dir[old] = make_uint2(p, min(c, pd.chunk_recs));
-          uint32_t nc = alloc_chunk(pd, blockIdx.x);
-          if(nc == NO_CHUNK) { atomicAdd(&a.T.stats[STAT_POOL_FULL], 1ull); st_chunk[p] = NO_CHUNK; st_cnt[p] = pd.chunk_recs; }
-          else { st_chunk[p] = nc; st_cnt[p] = 0; }
-        }
-      }
-    }
+    if(MODE == 2 && !FAST) for(uint32_t p = tid; p < pd.P; p += NTH) roll_chunk(pd, p, a.T.stats, st_chunk, st_cnt);
     __syncthreads();
   }
   if(MODE == 2) {          // keep the open chunks for the next launch

@@ -385,12 +385,45 @@ __device__ __forceinline__ uint32_t alloc_chunk(const PartDev& pd, uint32_t aren
   const uint32_t local = atomicAdd(&pd.pool_next[arena], 1u);
   return local < pd.arena_chunks ? arena * pd.arena_chunks + local : NO_CHUNK;
 }
+// a fresh chunk from `arena` for a region, with f = 0 records in it; when the arena is exhausted NO_CHUNK, and f = chunk_recs
+// sends the region's records to the spill list
+__device__ __forceinline__ uint32_t fresh_chunk(const PartDev& pd, uint32_t arena, unsigned long long* stats, uint32_t& f) {
+  const uint32_t c = alloc_chunk(pd, arena); f = 0;
+  if(c == NO_CHUNK) { atomicAdd(&stats[STAT_POOL_FULL], 1ull); f = pd.chunk_recs; }
+  return c;
+}
+// between two barriers of the staging kernels: close region p's open chunk once fewer than `margin` records are free in it
+// and open the next one of this CTA's arena
+__device__ __forceinline__ void roll_chunk(const PartDev& pd, uint32_t p, unsigned long long* stats, uint32_t* st_chunk, uint32_t* st_cnt) {
+  const uint32_t c = st_cnt[p];
+  if(c + pd.margin > pd.chunk_recs) {
+    const uint32_t old = st_chunk[p];
+    if(old != NO_CHUNK) pd.dir[old] = make_uint2(p, min(c, pd.chunk_recs));
+    uint32_t nc = alloc_chunk(pd, blockIdx.x);
+    if(nc == NO_CHUNK) { atomicAdd(&stats[STAT_POOL_FULL], 1ull); st_chunk[p] = NO_CHUNK; st_cnt[p] = pd.chunk_recs; }
+    else { st_chunk[p] = nc; st_cnt[p] = 0; }
+  }
+}
 __device__ __forceinline__ bool chunk_in_use(const PartDev& pd, uint32_t i) {
   const uint32_t a = i / pd.arena_chunks;
   return i - a * pd.arena_chunks < pd.pool_next[a];
 }
 
-__device__ __forceinline__ void store_rec(uint8_t* base, uint32_t rec_bytes, uint64_t idx, u128 r) {
+// A region record is (position inside the region << hb) | explicit key bits, hb = fbits - rbits; it is stored in
+// rec_bytes = 4, 8 or 16 bytes.
+__device__ __forceinline__ u128 rec_make(u128 high, uint64_t rel, uint32_t hb) {
+  u128 rec;
+  if(hb == 0)       { rec.lo = rel; rec.hi = 0; }
+  else if(hb < 64)  { rec.lo = high.lo | (rel << hb); rec.hi = high.hi | (rel >> (64 - hb)); }
+  else              { rec.lo = high.lo; rec.hi = high.hi | (rel << (hb - 64)); }
+  return rec;
+}
+__device__ __forceinline__ void rec_split(u128 rec, uint32_t hb, u128& high, uint64_t& rel) {
+  if(hb == 0)      { rel = rec.lo; high.lo = 0; high.hi = 0; }
+  else if(hb < 64) { high.lo = rec.lo & ((1ull << hb) - 1ull); high.hi = 0; rel = (rec.lo >> hb) | (rec.hi << (64 - hb)); }
+  else             { high.lo = rec.lo; high.hi = hb == 64 ? 0 : (rec.hi & ((1ull << (hb - 64)) - 1ull)); rel = hb == 64 ? rec.hi : (rec.hi >> (hb - 64)); }
+}
+__device__ __forceinline__ void store_rec(uint8_t* base, uint32_t rec_bytes, uint32_t idx, u128 r) {
   if(rec_bytes == 4) reinterpret_cast<uint32_t*>(base)[idx] = (uint32_t)r.lo;
   else if(rec_bytes == 8) reinterpret_cast<uint64_t*>(base)[idx] = r.lo;
   else { reinterpret_cast<uint64_t*>(base)[2 * idx] = r.lo; reinterpret_cast<uint64_t*>(base)[2 * idx + 1] = r.hi; }
@@ -500,11 +533,8 @@ __global__ void __launch_bounds__(512, 2) insert_chunks_kernel(TableDev T, PartD
 #pragma unroll
     for(int r = 0; r < 4; ++r) {
       valid[r] = (uint32_t)r < per16 && cur.v0 * per16 + r < cur.n_rec;
-      const u128 rec = recs[r];
       uint64_t rel;
-      if(hb == 0)      { rel = rec.lo; high[r].lo = 0; high[r].hi = 0; }
-      else if(hb < 64) { high[r].lo = rec.lo & ((1ull << hb) - 1ull); high[r].hi = 0; rel = (rec.lo >> hb) | (rec.hi << (64 - hb)); }
-      else             { high[r].lo = rec.lo; high[r].hi = hb == 64 ? 0 : (rec.hi & ((1ull << (hb - 64)) - 1ull)); rel = hb == 64 ? rec.hi : (rec.hi >> (hb - 64)); }
+      rec_split(recs[r], hb, high[r], rel);
       base[r] = cur.region_base + rel;
     }
     table_add_batch<SB, 4>(T, base, high, valid, ok, ls);
@@ -512,30 +542,13 @@ __global__ void __launch_bounds__(512, 2) insert_chunks_kernel(TableDev T, PartD
     for(int r = 0; r < 4; ++r) {
       if(!valid[r]) continue;
       if(ok[r]) { ls.inserted++; continue; }
-      // hash full: rebuild the key (low bits = inverse matrix * [explicit bits : position]) for the failure list
-      uint64_t v[KW], key[KW];
-      const uint64_t gpos = ((uint64_t)T.shard_index << T.local_lsize) | base[r];
-      v[0] = (T.lsize >= 64 ? 0 : (high[r].lo << T.lsize)) | gpos;
-      if(KW == 2) v[KW - 1] = T.lsize ? ((high[r].hi << T.lsize) | (high[r].lo >> (64 - T.lsize))) : high[r].hi;
-      const uint64_t low = gf2_hash<KW>(inv_lut_g, v, (int)nbytes);
-      const uint64_t lmask = T.lsize >= 64 ? ~0ull : ((1ull << T.lsize) - 1ull);
-#pragma unroll
-      for(int q = 0; q < KW; ++q) key[q] = v[q];
-      key[0] = (key[0] & ~lmask) | (low & lmask);
+      // hash full: rebuild the key for the failure list
+      uint64_t key[KW];
+      key_from_position<KW>(inv_lut_g, nbytes, T.lsize, high[r], global_pos(T, base[r]), key);
       record_failure<KW>(T, key, 1);
     }
   }
-  unsigned long long v[3] = { ls.inserted, ls.distinct, ls.reprobes };
-#pragma unroll
-  for(int q = 0; q < 3; ++q) {
-#pragma unroll
-    for(int o = 16; o; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
-  }
-  if(lane == 0) {
-    if(v[0]) atomicAdd(&T.stats[STAT_INSERTED], v[0]);
-    if(v[1]) atomicAdd(&T.stats[STAT_DISTINCT], v[1]);
-    if(v[2]) atomicAdd(&T.stats[STAT_REPROBES], v[2]);
-  }
+  flush_stats(T.stats, ls.inserted, ls.distinct, ls.reprobes);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -555,10 +568,7 @@ __global__ void __launch_bounds__(1024, 1) stage_keys_kernel(TableDev T, PartDev
   uint32_t* my_fill  = pd.cta_fill + (size_t)blockIdx.x * pd.P;
   for(uint32_t p = tid; p < pd.P; p += blockDim.x) {
     uint32_t c = my_chunk[p], f = my_fill[p];
-    if(c == NO_CHUNK) {
-      c = alloc_chunk(pd, blockIdx.x); f = 0;
-      if(c == NO_CHUNK) { atomicAdd(&T.stats[STAT_POOL_FULL], 1ull); f = pd.chunk_recs; }
-    }
+    if(c == NO_CHUNK) c = fresh_chunk(pd, blockIdx.x, T.stats, f);
     st_chunk[p] = c; st_cnt[p] = f;
   }
   __syncthreads();
@@ -578,18 +588,10 @@ __global__ void __launch_bounds__(1024, 1) stage_keys_kernel(TableDev T, PartDev
       const uint64_t lpos = pos & T.local_mask;
       const uint32_t p = (uint32_t)(lpos >> pd.region_bits);
       const uint64_t rel = lpos & ((1ull << pd.region_bits) - 1ull);
-      const u128 high = key_high<KW>(key, T.lsize);
-      u128 rec;
-      if(hb == 0)       { rec.lo = rel; rec.hi = 0; }
-      else if(hb < 64)  { rec.lo = high.lo | (rel << hb); rec.hi = high.hi | (rel >> (64 - hb)); }
-      else              { rec.lo = high.lo; rec.hi = high.hi | (rel << (hb - 64)); }
+      const u128 rec = rec_make(key_high<KW>(key, T.lsize), rel, hb);
       const uint32_t slot = atomicAdd(&st_cnt[p], 1u);
-      if(slot < pd.chunk_recs) {
-        uint8_t* dst = pd.pool + (size_t)st_chunk[p] * CHUNK_BYTES;
-        if(pd.rec_bytes == 4) reinterpret_cast<uint32_t*>(dst)[slot] = (uint32_t)rec.lo;
-        else if(pd.rec_bytes == 8) reinterpret_cast<uint64_t*>(dst)[slot] = rec.lo;
-        else { reinterpret_cast<uint64_t*>(dst)[2 * slot] = rec.lo; reinterpret_cast<uint64_t*>(dst)[2 * slot + 1] = rec.hi; }
-      } else {
+      if(slot < pd.chunk_recs) store_rec(pd.pool + (size_t)st_chunk[p] * CHUNK_BYTES, pd.rec_bytes, slot, rec);
+      else {
         unsigned long long at = atomicAdd(pd.spill_n, 1ull);
         if(at < pd.spill_cap) {
 #pragma unroll
@@ -599,16 +601,7 @@ __global__ void __launch_bounds__(1024, 1) stage_keys_kernel(TableDev T, PartDev
       }
     }
     __syncthreads();
-    for(uint32_t p = tid; p < pd.P; p += blockDim.x) {
-      const uint32_t c = st_cnt[p];
-      if(c + pd.margin > pd.chunk_recs) {
-        const uint32_t old = st_chunk[p];
-        if(old != NO_CHUNK) pd.dir[old] = make_uint2(p, min(c, pd.chunk_recs));
-        uint32_t nc = alloc_chunk(pd, blockIdx.x);
-        if(nc == NO_CHUNK) { atomicAdd(&T.stats[STAT_POOL_FULL], 1ull); st_chunk[p] = NO_CHUNK; st_cnt[p] = pd.chunk_recs; }
-        else { st_chunk[p] = nc; st_cnt[p] = 0; }
-      }
-    }
+    for(uint32_t p = tid; p < pd.P; p += blockDim.x) roll_chunk(pd, p, T.stats, st_chunk, st_cnt);
     __syncthreads();
   }
   for(uint32_t p = tid; p < pd.P; p += blockDim.x) { my_chunk[p] = st_chunk[p]; my_fill[p] = min(st_cnt[p], pd.chunk_recs); }
@@ -622,15 +615,10 @@ template<int KW>
 __device__ __noinline__ void k2_fail(uint32_t shard_index, uint32_t local_lsize, uint32_t lsize, unsigned long long* stats,
                                      uint64_t* fail_keys, uint64_t* fail_counts, uint64_t fail_cap,
                                      uint64_t base, uint32_t high, const uint64_t* inv_lut_g, uint32_t nbytes) {
-  uint64_t v[KW], key[KW];
-  const uint64_t gpos = ((uint64_t)shard_index << local_lsize) | base;
-  v[0] = (lsize >= 64 ? 0 : ((uint64_t)high << lsize)) | gpos;
-  if(KW == 2) v[KW - 1] = lsize ? ((uint64_t)high >> (64 - lsize)) : 0;
-  const uint64_t low = gf2_hash<KW>(inv_lut_g, v, (int)nbytes);
-  const uint64_t lmask = lsize >= 64 ? ~0ull : ((1ull << lsize) - 1ull);
-#pragma unroll
-  for(int q = 0; q < KW; ++q) key[q] = v[q];
-  key[0] = (key[0] & ~lmask) | (low & lmask);
+  // (everything by value, as for spill_record; so the global position is spelled out here rather than taken from global_pos)
+  uint64_t key[KW];
+  const u128 h = { high, 0 };
+  key_from_position<KW>(inv_lut_g, nbytes, lsize, h, ((uint64_t)shard_index << local_lsize) | base, key);
   unsigned long long at = atomicAdd(&stats[STAT_FAILED], 1ull);
   if(at < fail_cap) {
 #pragma unroll
@@ -672,13 +660,39 @@ __device__ __noinline__ uint32_t k2_walk(uint32_t* tab, uint64_t base, uint32_t 
   return 0;
 }
 
+// one record of a 32-bit table (slot `base`, explicit key bits `high`) after the CAS of its first probe returned `old`: a
+// new key, an increment of the same key (its carry to the side table), or the rest of the probe sequence (k2_walk); a key
+// that finds no slot goes to the failure list
+template<int KW>
+__device__ __forceinline__ void k2_settle(const TableDev& T, uint32_t* tab, uint64_t base, uint32_t high, uint32_t old,
+                                          const uint64_t* inv_lut_g, uint32_t nbytes, uint32_t& n_ins, uint32_t& n_new, uint32_t& n_rep) {
+  const uint32_t fb = T.fbits, kf0 = high << T.rbits;
+  const uint32_t fmask = (1u << fb) - 1u, one = 1u << fb, cb = 32 - fb;
+  bool ok = true;
+  if(old == 0u) ++n_new;
+  else if((old & fmask) == (kf0 | 1u)) {
+    const uint32_t o2 = atomicAdd(&tab[base], one);
+    if((((o2 >> fb) + 1) >> cb) != 0) k2_carry(T.ovf_keys, T.ovf_vals, T.ovf_mask, T.stats, base);
+  } else {
+    const uint32_t w = k2_walk(tab, base, kf0, fb, T.max_reprobe);
+    ok = w != 0;
+    if(ok) {
+      const uint32_t i = (w & 0xFFFFu) - 1;
+      n_rep += i; if(w & 0x10000u) ++n_new;
+      if(w & 0x20000u) k2_carry(T.ovf_keys, T.ovf_vals, T.ovf_mask, T.stats, base + tri(i));
+    }
+  }
+  if(ok) ++n_ins;
+  else k2_fail<KW>(T.shard_index, T.local_lsize, T.lsize, T.stats, T.fail_keys, T.fail_counts, T.fail_cap, base, high, inv_lut_g, nbytes);
+}
+
 template<int KW>
 __global__ void __launch_bounds__(768, 2) insert_chunks32_kernel(TableDev T, PartDev pd, const uint32_t* __restrict__ order,
                                                                    unsigned int* __restrict__ piece_cursor, uint32_t from, uint32_t upto,
                                                                    const uint64_t* __restrict__ inv_lut_g, uint32_t nbytes) {
   const uint32_t n_units = min(*pd.n_units, upto);
   const uint32_t fb = T.fbits, rb = T.rbits, hb = fb - rb;
-  const uint32_t fmask = (1u << fb) - 1u, one = 1u << fb, cb = 32 - fb;
+  const uint32_t one = 1u << fb;
   const uint32_t hmask = hb ? ((1u << hb) - 1u) : 0u;
   const uint32_t lane = threadIdx.x & 31;
   uint32_t* tab = (uint32_t*)T.slots;
@@ -717,37 +731,11 @@ __global__ void __launch_bounds__(768, 2) insert_chunks32_kernel(TableDev T, Par
 #pragma unroll
     for(int r = 0; r < 4; ++r) {
       if((uint32_t)r >= nv) continue;
-      const uint32_t kf0 = (rec[r] & hmask) << rb;
-      const uint64_t base = rbase + (hb < 32 ? rec[r] >> hb : 0u);
-      bool ok = true;
-      if(old[r] == 0u) n_new++;
-      else if((old[r] & fmask) == (kf0 | 1u)) {
-        const uint32_t o2 = atomicAdd(&tab[base], one);
-        if((((o2 >> fb) + 1) >> cb) != 0) k2_carry(T.ovf_keys, T.ovf_vals, T.ovf_mask, T.stats, base);
-      } else {
-        const uint32_t w = k2_walk(tab, base, kf0, fb, T.max_reprobe);
-        ok = w != 0;
-        if(ok) {
-          const uint32_t i = (w & 0xFFFFu) - 1;
-          n_rep += i; if(w & 0x10000u) n_new++;
-          if(w & 0x20000u) k2_carry(T.ovf_keys, T.ovf_vals, T.ovf_mask, T.stats, base + tri(i));
-        }
-      }
-      if(ok) n_ins++;
-      else k2_fail<KW>(T.shard_index, T.local_lsize, T.lsize, T.stats, T.fail_keys, T.fail_counts, T.fail_cap, base, rec[r] & hmask, inv_lut_g, nbytes);
+      const uint32_t high = rec[r] & hmask;
+      k2_settle<KW>(T, tab, rbase + (hb < 32 ? rec[r] >> hb : 0u), high, old[r], inv_lut_g, nbytes, n_ins, n_new, n_rep);
     }
   }
-  unsigned long long v[3] = { n_ins, n_new, n_rep };
-#pragma unroll
-  for(int q = 0; q < 3; ++q) {
-#pragma unroll
-    for(int o = 16; o; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
-  }
-  if(lane == 0) {
-    if(v[0]) atomicAdd(&T.stats[STAT_INSERTED], v[0]);
-    if(v[1]) atomicAdd(&T.stats[STAT_DISTINCT], v[1]);
-    if(v[2]) atomicAdd(&T.stats[STAT_REPROBES], v[2]);
-  }
+  flush_stats(T.stats, n_ins, n_new, n_rep);
 }
 
 // After a regrow in the middle of a drain: the remaining records still describe positions of
@@ -778,36 +766,16 @@ __global__ void __launch_bounds__(512, 1) rehash_chunks_kernel(TableDev T, Table
     const uint8_t* src = pd.pool + (size_t)chunk * CHUNK_BYTES;
     const uint64_t region_base = (uint64_t)d.x << pd.region_bits;
     for(uint32_t i = threadIdx.x; i < d.y; i += blockDim.x) {
-      const u128 rec = load_rec(src, pd.rec_bytes, i);
       u128 high; uint64_t rel;
-      if(hb == 0)      { rel = rec.lo; high.lo = 0; high.hi = 0; }
-      else if(hb < 64) { high.lo = rec.lo & ((1ull << hb) - 1ull); high.hi = 0; rel = (rec.lo >> hb) | (rec.hi << (64 - hb)); }
-      else             { high.lo = rec.lo; high.hi = hb == 64 ? 0 : (rec.hi & ((1ull << (hb - 64)) - 1ull)); rel = hb == 64 ? rec.hi : (rec.hi >> (hb - 64)); }
-      const uint64_t gpos = ((uint64_t)T0.shard_index << T0.local_lsize) | (region_base + rel);
-      uint64_t v[KW], key[KW];
-      v[0] = (T0.lsize >= 64 ? 0 : (high.lo << T0.lsize)) | gpos;
-      if(KW == 2) v[KW - 1] = T0.lsize ? ((high.hi << T0.lsize) | (high.lo >> (64 - T0.lsize))) : high.hi;
-      const uint64_t low = gf2_hash<KW>(inv, v, (int)nbytes);
-      const uint64_t lmask = T0.lsize >= 64 ? ~0ull : ((1ull << T0.lsize) - 1ull);
-#pragma unroll
-      for(int q = 0; q < KW; ++q) key[q] = v[q];
-      key[0] = (key[0] & ~lmask) | (low & lmask);
+      rec_split(load_rec(src, pd.rec_bytes, i), hb, high, rel);
+      uint64_t key[KW];
+      key_from_position<KW>(inv, nbytes, T0.lsize, high, global_pos(T0, region_base + rel), key);
       const uint64_t pos = gf2_hash<KW>(lut, key, (int)nbytes);
       if(table_add<KW, SB>(T, key, pos, 1, ls)) ls.inserted++;
       else record_failure<KW>(T, key, 1);
     }
   }
-  unsigned long long v[3] = { ls.inserted, ls.distinct, ls.reprobes };
-#pragma unroll
-  for(int q = 0; q < 3; ++q) {
-#pragma unroll
-    for(int o = 16; o; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
-  }
-  if((threadIdx.x & 31) == 0) {
-    if(v[0]) atomicAdd(&T.stats[STAT_INSERTED], v[0]);
-    if(v[1]) atomicAdd(&T.stats[STAT_DISTINCT], v[1]);
-    if(v[2]) atomicAdd(&T.stats[STAT_REPROBES], v[2]);
-  }
+  flush_stats(T.stats, ls.inserted, ls.distinct, ls.reprobes);
 }
 
 // insert the spilled keys (count taken from device memory so that no host round trip is needed)
@@ -828,17 +796,7 @@ __global__ void __launch_bounds__(256) insert_spill_kernel(TableDev T, const uin
     if(table_add<KW, SB>(T, key, pos, pd.spill_counts[i], ls)) occ += pd.spill_counts[i];
     else record_failure<KW>(T, key, pd.spill_counts[i]);
   }
-  unsigned long long v[3] = { occ, ls.distinct, ls.reprobes };
-#pragma unroll
-  for(int q = 0; q < 3; ++q) {
-#pragma unroll
-    for(int o = 16; o; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
-  }
-  if((threadIdx.x & 31) == 0) {
-    if(v[0]) atomicAdd(&T.stats[STAT_INSERTED], v[0]);
-    if(v[1]) atomicAdd(&T.stats[STAT_DISTINCT], v[1]);
-    if(v[2]) atomicAdd(&T.stats[STAT_REPROBES], v[2]);
-  }
+  flush_stats(T.stats, occ, ls.distinct, ls.reprobes);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -863,17 +821,7 @@ __global__ void __launch_bounds__(256) insert_keys_kernel(TableDev T, const uint
     if(table_add<KW, SB>(T, key, pos, cnt, ls)) occ += cnt;
     else { ls.failed++; record_failure<KW>(T, key, cnt); }
   }
-  unsigned long long v[3] = { occ, ls.distinct, ls.reprobes };
-#pragma unroll
-  for(int q = 0; q < 3; ++q) {
-#pragma unroll
-    for(int o = 16; o; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
-  }
-  if((threadIdx.x & 31) == 0) {
-    if(v[0]) atomicAdd(&T.stats[STAT_INSERTED], v[0]);
-    if(v[1]) atomicAdd(&T.stats[STAT_DISTINCT], v[1]);
-    if(v[2]) atomicAdd(&T.stats[STAT_REPROBES], v[2]);
-  }
+  flush_stats(T.stats, occ, ls.distinct, ls.reprobes);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -919,15 +867,7 @@ __global__ void __launch_bounds__(256) collect_kernel(const CollectArgs a) {
     if(i < span && slot_decode<SB>(T, idx, high, rp, cnt)) {
       opos = idx - (rp ? tri(rp) : 0);
       if(opos >= a.seg_lo && opos < a.seg_hi) {
-        if(T.stats[STAT_OVERFLOWED]) {
-          const uint32_t cb = slot_counter_bits<SB>(T);
-          const uint64_t carries = ovf_get(T, idx);
-          if(carries) {
-            // saturate at 2^64-1 like a 64-bit counter would
-            if(cb >= 64 || (carries >> (64 - cb)) != 0) cnt = ~0ull;
-            else { uint64_t add = carries << cb; cnt = (cnt + add < cnt) ? ~0ull : cnt + add; }
-          }
-        }
+        if(T.stats[STAT_OVERFLOWED]) cnt = slot_full_count<SB>(T, idx, cnt);
         have = cnt >= a.lower && cnt <= a.upper;
       }
     }
@@ -947,21 +887,8 @@ __global__ void __launch_bounds__(256) collect_kernel(const CollectArgs a) {
             a.out_sort_lo[o] = opos - a.seg_lo;
           }
         } else if(o < a.out_cap) {
-          // global position = shard bits : local original position
-          const uint64_t gpos = ((uint64_t)T.shard_index << T.local_lsize) | opos;
-          // vector fed to the inverse matrix: [high bits of key : position]
-          uint64_t v[KW];
-          if(KW == 1) v[0] = (T.lsize >= 64 ? 0 : (high.lo << T.lsize)) | gpos;
-          else {
-            v[0] = (T.lsize >= 64 ? 0 : (high.lo << T.lsize)) | gpos;
-            v[KW - 1] = T.lsize ? ((high.hi << T.lsize) | (high.lo >> (64 - T.lsize))) : high.hi;
-          }
-          const uint64_t low = gf2_hash<KW>(lut, v, (int)a.nbytes);
-          const uint64_t lmask = T.lsize >= 64 ? ~0ull : ((1ull << T.lsize) - 1ull);
           uint64_t key[KW];
-#pragma unroll
-          for(int q = 0; q < KW; ++q) key[q] = v[q];
-          key[0] = (key[0] & ~lmask) | (low & lmask);
+          key_from_position<KW>(lut, a.nbytes, T.lsize, high, global_pos(T, opos), key);
 #pragma unroll
           for(int q = 0; q < KW; ++q) a.out_keys[o * KW + q] = key[q];
           a.out_counts[o] = cnt;
@@ -993,13 +920,7 @@ __device__ __forceinline__ uint64_t table_get(const TableDev& T, const uint64_t 
   if constexpr(SB == SB_WIDE) {
     uint64_t idx = 0, cnt = 0;
     if(!wide_find(T, pos & T.local_mask, key, idx, cnt)) return 0;
-    const uint32_t cb = slot_counter_bits<SB>(T);
-    const uint64_t carries = T.stats[STAT_OVERFLOWED] ? ovf_get(T, idx) : 0;
-    if(carries) {
-      if((carries >> (64 - cb)) != 0) cnt = ~0ull;
-      else { uint64_t add = carries << cb; cnt = (cnt + add < cnt) ? ~0ull : cnt + add; }
-    }
-    return cnt;
+    return T.stats[STAT_OVERFLOWED] ? slot_full_count<SB>(T, idx, cnt) : cnt;
   }
   const u128 want = key_high<KW>(key, T.lsize);
   const uint64_t base = pos & T.local_mask;
@@ -1008,12 +929,7 @@ __device__ __forceinline__ uint64_t table_get(const TableDev& T, const uint64_t 
     u128 high; uint32_t rp; uint64_t cnt;
     if(!slot_decode<SB>(T, idx, high, rp, cnt)) break;          // empty slot ends the probe sequence
     if(rp == r && high.lo == want.lo && high.hi == want.hi) {
-      const uint32_t cb = slot_counter_bits<SB>(T);
-      const uint64_t carries = T.stats[STAT_OVERFLOWED] ? ovf_get(T, idx) : 0;
-      if(carries) {
-        if(cb >= 64 || (carries >> (64 - cb)) != 0) cnt = ~0ull;
-        else { uint64_t add = carries << cb; cnt = (cnt + add < cnt) ? ~0ull : cnt + add; }
-      }
+      if(T.stats[STAT_OVERFLOWED]) cnt = slot_full_count<SB>(T, idx, cnt);
       return cnt;
     }
     idx = base + tri(r + 1);
@@ -1043,14 +959,7 @@ __global__ void __launch_bounds__(256) histogram_kernel(TableDev T, uint64_t n_s
   for(uint64_t idx = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < n_slots; idx += (uint64_t)gridDim.x * blockDim.x) {
     u128 high; uint32_t rp; uint64_t cnt;
     if(slot_decode<SB>(T, idx, high, rp, cnt)) {
-      if(T.stats[STAT_OVERFLOWED]) {
-        const uint32_t cb = slot_counter_bits<SB>(T);
-        const uint64_t carries = ovf_get(T, idx);
-        if(carries) {
-          if(cb >= 64 || (carries >> (64 - cb)) != 0) cnt = ~0ull;
-          else { uint64_t add = carries << cb; cnt = (cnt + add < cnt) ? ~0ull : cnt + add; }
-        }
-      }
+      if(T.stats[STAT_OVERFLOWED]) cnt = slot_full_count<SB>(T, idx, cnt);
       atomicAdd(&hist[cnt < n_bins ? cnt : n_bins - 1], 1ull);
     }
   }
@@ -1062,14 +971,7 @@ __global__ void __launch_bounds__(256) max_count_kernel(TableDev T, uint64_t n_s
   for(uint64_t idx = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < n_slots; idx += (uint64_t)gridDim.x * blockDim.x) {
     u128 high; uint32_t rp; uint64_t cnt;
     if(slot_decode<SB>(T, idx, high, rp, cnt)) {
-      if(T.stats[STAT_OVERFLOWED]) {
-        const uint32_t cb = slot_counter_bits<SB>(T);
-        const uint64_t carries = ovf_get(T, idx);
-        if(carries) {
-          if(cb >= 64 || (carries >> (64 - cb)) != 0) cnt = ~0ull;
-          else { uint64_t add = carries << cb; cnt = (cnt + add < cnt) ? ~0ull : cnt + add; }
-        }
-      }
+      if(T.stats[STAT_OVERFLOWED]) cnt = slot_full_count<SB>(T, idx, cnt);
       m = max(m, (unsigned long long)cnt);
     }
   }

@@ -46,10 +46,7 @@ __global__ void __launch_bounds__(1024, 1) restage_kernel(const RestageArgs ra, 
   uint32_t* my_fill  = pd.cta_fill + (size_t)blockIdx.x * pd.P;
   for(uint32_t p = tid; p < pd.P; p += NTH) {
     uint32_t c = my_chunk[p], f = my_fill[p];
-    if(c == NO_CHUNK) {
-      c = alloc_chunk(pd, blockIdx.x); f = 0;
-      if(c == NO_CHUNK) { atomicAdd(&T.stats[STAT_POOL_FULL], 1ull); f = pd.chunk_recs; }
-    }
+    if(c == NO_CHUNK) c = fresh_chunk(pd, blockIdx.x, T.stats, f);
     st_chunk[p] = c; st_cnt[p] = f | (f << 16);
   }
   __syncthreads();
@@ -152,17 +149,7 @@ __global__ void __launch_bounds__(1024, 1) restage_kernel(const RestageArgs ra, 
   flush_rings(true);
   __syncthreads();
   for(uint32_t p = tid; p < pd.P; p += NTH) { my_chunk[p] = st_chunk[p]; my_fill[p] = min(st_cnt[p] & 0xFFFFu, pd.chunk_recs); }
-  unsigned long long v[3] = { ls.inserted, ls.distinct, ls.reprobes };
-#pragma unroll
-  for(int q = 0; q < 3; ++q) {
-#pragma unroll
-    for(int o = 16; o; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
-  }
-  if((tid & 31) == 0) {
-    if(v[0]) atomicAdd(&T.stats[STAT_INSERTED], v[0]);
-    if(v[1]) atomicAdd(&T.stats[STAT_DISTINCT], v[1]);
-    if(v[2]) atomicAdd(&T.stats[STAT_REPROBES], v[2]);
-  }
+  flush_stats(T.stats, ls.inserted, ls.distinct, ls.reprobes);
 }
 
 }  // namespace jfk

@@ -367,17 +367,7 @@ __global__ void __launch_bounds__(WIN2_NTH, 1) win_insert2_kernel(TableDev T, Pa
       if(lane == 0) mbar_arrive(&empty[s]);        // this warp is done with the batch
     }
   }
-  unsigned long long v[3] = { n_ins, n_new, n_rep };
-#pragma unroll
-  for(int q = 0; q < 3; ++q) {
-#pragma unroll
-    for(int o = 16; o; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
-  }
-  if(lane == 0) {
-    if(v[0]) atomicAdd(&T.stats[STAT_INSERTED], v[0]);
-    if(v[1]) atomicAdd(&T.stats[STAT_DISTINCT], v[1]);
-    if(v[2]) atomicAdd(&T.stats[STAT_REPROBES], v[2]);
-  }
+  flush_stats(T.stats, n_ins, n_new, n_rep);
 }
 
 // ---- lazily zeroed table: windows [w_first, w_first + n) that are not in memory yet are written as zeros, except those that
@@ -396,43 +386,17 @@ __global__ void __launch_bounds__(256) win_zero_kernel(uint32_t* __restrict__ ta
 // ---- the deferred records: ordinary probe sequence in global memory ---------------------------------
 template<int KW>
 __global__ void __launch_bounds__(256) win_deferred_kernel(TableDev T, WinDev wd, const uint64_t* __restrict__ inv_lut_g, uint32_t nbytes) {
-  const uint32_t fb = T.fbits, rb = T.rbits;
-  const uint32_t fmask = (1u << fb) - 1u, one = 1u << fb, cb = 32 - fb;
+  const uint32_t one = 1u << T.fbits;
   uint32_t* tab = (uint32_t*)T.slots;
   const unsigned long long n = min(*wd.def_n, (unsigned long long)wd.def_cap);
   uint32_t n_ins = 0, n_new = 0, n_rep = 0;
   for(unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
     const uint64_t base = wd.def_pos[i];
-    const uint32_t high = wd.def_high[i], kf0 = high << rb;
-    bool ok = true;
-    const uint32_t o = atomicCAS(&tab[base], 0u, (kf0 | 1u) | one);
-    if(o == 0u) ++n_new;
-    else if((o & fmask) == (kf0 | 1u)) {
-      const uint32_t o2 = atomicAdd(&tab[base], one);
-      if((((o2 >> fb) + 1) >> cb) != 0) k2_carry(T.ovf_keys, T.ovf_vals, T.ovf_mask, T.stats, base);
-    } else {
-      const uint32_t w = k2_walk(tab, base, kf0, fb, T.max_reprobe);
-      ok = w != 0;
-      if(ok) {
-        const uint32_t p = (w & 0xFFFFu) - 1;
-        n_rep += p; if(w & 0x10000u) ++n_new;
-        if(w & 0x20000u) k2_carry(T.ovf_keys, T.ovf_vals, T.ovf_mask, T.stats, base + tri(p));
-      }
-    }
-    if(ok) ++n_ins;
-    else k2_fail<KW>(T.shard_index, T.local_lsize, T.lsize, T.stats, T.fail_keys, T.fail_counts, T.fail_cap, base, high, inv_lut_g, nbytes);
+    const uint32_t high = wd.def_high[i];
+    const uint32_t o = atomicCAS(&tab[base], 0u, ((high << T.rbits) | 1u) | one);
+    k2_settle<KW>(T, tab, base, high, o, inv_lut_g, nbytes, n_ins, n_new, n_rep);
   }
-  unsigned long long v[3] = { n_ins, n_new, n_rep };
-#pragma unroll
-  for(int q = 0; q < 3; ++q) {
-#pragma unroll
-    for(int o2 = 16; o2; o2 >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o2);
-  }
-  if((threadIdx.x & 31) == 0) {
-    if(v[0]) atomicAdd(&T.stats[STAT_INSERTED], v[0]);
-    if(v[1]) atomicAdd(&T.stats[STAT_DISTINCT], v[1]);
-    if(v[2]) atomicAdd(&T.stats[STAT_REPROBES], v[2]);
-  }
+  flush_stats(T.stats, n_ins, n_new, n_rep);
 }
 
 }  // namespace jfk
