@@ -225,14 +225,17 @@ int table_setup(jfgpu_engine* e, Table& t, unsigned lsize, const jfb::gf2_matrix
   for(unsigned i = 0; i <= limit; ++i) t.reprobes[i] = rp(i);
   t.rbits = bitsize(limit + 1);
   t.fbits = t.hb + t.rbits;
-  // at least 10 counter bits in a slot, so that only counts beyond ~1000 need the carry side table
+  // the narrowest slot that keeps at least 8 counter bits, so that only counts beyond ~250 need the carry side table; a
+  // 128-bit slot also takes key fields of 121..127 bits (k = 61..64 in tables of at most 2^14 slots), whose 1..7-bit counter
+  // carries into the side table on nearly every increment (it has at least 2^20 entries, such a table at most 2^14 slots)
   if(e->kw == 4) {                 // four-word keys: the wide form, the whole key beside a head word (jf_device.cuh, SB_WIDE)
     t.fbits = t.rbits + 1;         // the head's low bits: reprobe+1 and READY
     t.slot_bits = SB_WIDE;
   } else if(t.fbits <= 22) t.slot_bits = 32;
   else if(t.fbits <= 56) t.slot_bits = 64;
-  else if(t.fbits <= 120) t.slot_bits = 128;
-  else return fail(e, JFGPU_ERR_ARG, "key too long for this table size (key field > 120 bits)");
+  else if(t.fbits <= 127) t.slot_bits = 128;
+  else return fail(e, JFGPU_ERR_ARG, "key too long for this table size (k=" + std::to_string(e->k) + ", " + std::to_string(t.size) +
+                                     " slots: a key field of " + std::to_string(t.fbits) + " bits, at most 127 fit a slot)");
   if(e->kw == 2 && t.slot_bits == 32) t.slot_bits = 64;
   t.margin = limit ? tri(limit) : 0;
   t.local_slots = t.local_size + t.margin + 8;
@@ -456,6 +459,8 @@ void part_configure(jfgpu_engine* e) {
     const uint32_t region_bits = t.local_lsize - ceil_log2(P);
     const uint32_t bits = region_bits + t.hb;
     const uint32_t rec = bits <= 32 ? 4 : bits <= 64 ? 8 : bits <= 128 ? 16 : 0;
+    // (a 16-byte record cannot hold hb + region_bits of a key field of 121..127 bits; those tables have at most 2^14
+    // 128-bit slots, below the 1 MB floor of part_min_mb, so they never get here)
     if(!rec) return;
     // records arriving per region between two roll-over passes (one per window): 1024 threads x 32 symbols / P
     const double mean = 1024.0 * 32 / P;
@@ -2118,7 +2123,8 @@ int jfgpu_load_records(jfgpu_handle e, const void* records, size_t nbytes, uint3
   cudaStreamSynchronize(e->cs);
   raw.free(); keys.free(); counts.free();
   for(int i = 0; i < 2; ++i) if(h[i]) cudaFreeHost(h[i]);
-  if(rc == JFGPU_ERR_FULL) rc = fail(e, JFGPU_ERR_NOMEM, "the database does not fit in device memory (" + e->err + ")");
+  // (a full carry side table is not a lack of memory: a larger table would not get a larger one below 2^26 slots)
+  if(rc == JFGPU_ERR_FULL && !e->h_stats[STAT_OVF_FULL]) rc = fail(e, JFGPU_ERR_NOMEM, "the database does not fit in device memory (" + e->err + ")");
   return rc;
 }
 

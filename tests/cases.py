@@ -61,6 +61,12 @@ CASES = {
     "grow2":        (["-m", "21", "-s", "100k", "-C"], ["plain.fa"]),
     "grow_k40":     (["-m", "40", "-s", "50k"], ["plain.fa"]),
     "grow_to_full": (["-m", "8", "-s", "10k", "-C"], ["plain.fa"]),
+    # key fields of 121..127 bits (k = 62..64 in small tables: 128-bit slots with a 1..7-bit counter) that double out of
+    # that size; k = 63 and 62 start with a clipped reprobe limit (90, 31) and keep it through every doubling.  (k = 61 at
+    # -s 32 is no golden case: its limit of 7 makes the final size depend on the insertion order at a load near 0.3.)
+    "wide_key_k64": (["-m", "64", "-s", "16k", "-C"], ["multi2.fa"]),
+    "wide_key_k63": (["-m", "63", "-s", "4k", "-C"], ["multi2.fa"]),
+    "wide_key_k62": (["-m", "62", "-s", "512", "-C"], ["dangling.fa"]),
 }
 
 # -Q / --min-quality (count_main.cc:326-329: whole_sequence_parser + mer_qual_iterator). The
@@ -136,9 +142,13 @@ BC_CASES = {
 # a direct-indexed table (size = 4^k) grows val_len only when a continuation entry finds no slot.
 # The restatement reproduces all of these (reference run with -t 1); the device engine does not yet
 # (DESIGN.md section 7a), so these stay out of CASES.
+# A case's final size must not depend on the insertion order, or the reference with -t 1 and a GPU run can end one
+# doubling apart: k = 54 at -s 10 over multi2.fa (carried limit 5) fits its last table of 2^19 slots in about five of
+# six orders, k = 48 at -s 100 over multi.fa (limit 15) fits 2^19 slots in about one order of three (the reference
+# itself ends there with -t 8).  At -s 40 and -s 60 (limit 10) every order tried fits the final size and not half of it.
 EDGE_CASES = {
-    "edge_s100_k48":   (["-m", "48", "-s", "100", "-C"], ["multi.fa"]),
-    "edge_s10_k54":    (["-m", "54", "-s", "10"], ["multi2.fa"]),
+    "edge_s60_k48":    (["-m", "48", "-s", "60", "-C"], ["multi.fa"]),
+    "edge_s40_k54":    (["-m", "54", "-s", "40"], ["multi2.fa"]),
     "edge_s2_ties":    (["-m", "25", "-s", "2", "-C"], ["dangling.fa", "cr_mid.fa", "one_read.fq"]),
     "edge_s2_k31_p62": (["-m", "31", "-s", "2", "-C", "-p", "62"], ["multi2.fa"]),
     "edge_direct_sparse": (["-m", "4", "-s", "100k", "-C"], ["polya.fa", "dangling.fa"]),
