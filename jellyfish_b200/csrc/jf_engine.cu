@@ -375,7 +375,7 @@ size_t wide_extract_smem(size_t lut_bytes) { return jfw::extract_smem(lut_bytes)
 
 template<int NTH>
 size_t count_smem_bytes(size_t lut_bytes, size_t stage_bytes, size_t bloom_bytes = 0, bool fast = false) {
-  const size_t part = fast ? (size_t)RING_P * 8 + (size_t)RING_P * RING * 4 : (stage_bytes ? PMAX * 4 + stage_bytes : 0);
+  const size_t part = fast ? FAST_SMEM : (stage_bytes ? PMAX * 4 + stage_bytes : 0);
   return ((sizeof(ExtractSmemT<NTH>) + 15) & ~(size_t)15) + lut_bytes + part + bloom_bytes;
 }
 

@@ -107,10 +107,12 @@ __device__ __noinline__ void spill_record(const TableDev T, uint64_t* spill_keys
 // 11-bit-table hash with at most six parity rows (tables of up to 2^38 slots), 4-byte records, at most RING_P regions
 // (the regions of this GPU's table, or -- sharded counting -- of the GLOBAL table, chunks then grouped by owning shard).  Its records do not go to the chunks one 4-byte store at a time (the GPU retires ~98 G scattered stores
 // per second whatever their width, scripts/micro/scatter_store.cu -- that alone would cap K1 at 98 G k-mers/s): every region
-// has a ring of RING records in shared memory, and after every SG k-mers per thread a pass over the regions writes the
-// complete groups of 8 records with two 16-byte stores (one 32-byte sector).
+// has a ring of RING records in shared memory, and after every 8 k-mers per thread (SG on the sharded send side) a pass over
+// the regions writes the complete groups of 8 records with two 16-byte stores (one 32-byte sector).
 constexpr uint32_t RING = 32;                     // records per region ring with RING_P regions (PartDev::ring_len in general)
 constexpr uint32_t RING_P = 1024;                 // regions at most on the FAST path (shared memory: RING_P * RING * 4 bytes)
+// shared memory of the FAST tail behind the hash table: per region a counter, an open chunk id and a ring; then the arena cursor
+constexpr size_t FAST_SMEM = (size_t)RING_P * 8 + (size_t)RING_P * RING * 4 + 16;
 // NPR (FAST only): parity rows evaluated per k-mer -- 2 covers tables of up to 2^34 slots (unused rows are zero), 6 the
 // sharded tables of up to 2^38.
 template<int KW, int SB, int MODE, int NTH, bool FAST, int NPR = 2>
@@ -129,9 +131,15 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
   uint32_t* st_cnt = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(lut) + a.lut_bytes);
   uint32_t* st_chunk = st_cnt + (FAST ? RING_P : PMAX);
   uint32_t* ring = st_chunk + RING_P;            // (FAST only)
+  // FAST, single-GPU counting: the allocation cursor of this CTA's arena, kept here for the launch.  Arena blockIdx.x is this
+  // CTA's alone, and the K1 launches of one engine run one after the other on one stream (the open chunks in cta_chunk rely
+  // on that too), so closing a chunk costs a shared-memory atomic instead of a round trip to L2 while 1023 threads wait at
+  // the next barrier.  The sharded send side shares each owner's arena among all CTAs and keeps the global cursor.
+  unsigned int* arena_next = ring + RING_P * RING;
+  const bool own_arena = FAST && !pd.by_owner;
   // byte tables of the two Bloom hash matrices, behind everything else
   uint64_t* bl1 = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(lut) + a.lut_bytes +
-                                              (MODE == 2 ? (FAST ? (size_t)RING_P * 8 + (size_t)RING_P * RING * 4 : (size_t)PMAX * 8) : 0));
+                                              (MODE == 2 ? (FAST ? FAST_SMEM : (size_t)PMAX * 8) : 0));
   uint64_t* bl2 = bl1 + a.nbytes * 256;
   const uint32_t* lut32 = reinterpret_cast<const uint32_t*>(lut);
   const uint64_t* rev64 = reinterpret_cast<const uint64_t*>(sm.rev);
@@ -144,16 +152,35 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
   if(a.bloom.mode) for(uint32_t i = tid; i < a.nbytes * 256; i += NTH) { bl1[i] = a.bloom.lut1[i]; bl2[i] = a.bloom.lut2[i]; }
   uint32_t* my_chunk = MODE == 2 ? pd.cta_chunk + (size_t)blockIdx.x * pd.P : nullptr;
   uint32_t* my_fill  = MODE == 2 ? pd.cta_fill + (size_t)blockIdx.x * pd.P : nullptr;
+  // FAST: a fresh chunk for region p; NO_CHUNK when the arena is exhausted
+  auto take_chunk = [&](const uint32_t p) -> uint32_t {
+    if(!own_arena) return alloc_chunk(pd, pd.by_owner ? (p >> pd.owner_shift) : blockIdx.x);
+    const uint32_t local = atomicAdd(arena_next, 1u);
+    return local < pd.arena_chunks ? blockIdx.x * pd.arena_chunks + local : NO_CHUNK;
+  };
   if(MODE == 2) {
+    if(own_arena) {
+      if(tid == 0) *arena_next = pd.pool_next[blockIdx.x];
+      __syncthreads();
+    }
     for(uint32_t p = tid; p < pd.P; p += NTH) {
       uint32_t c = my_chunk[p], f = my_fill[p];
-      if(c == NO_CHUNK) c = fresh_chunk(pd, pd.by_owner ? (p >> pd.owner_shift) : blockIdx.x, a.T.stats, f);
+      if(c == NO_CHUNK) {
+        if constexpr(FAST) {
+          c = take_chunk(p); f = 0;
+          if(c == NO_CHUNK) { atomicAdd(&a.T.stats[STAT_POOL_FULL], 1ull); f = pd.chunk_recs; }
+        } else c = fresh_chunk(pd, pd.by_owner ? (p >> pd.owner_shift) : blockIdx.x, a.T.stats, f);
+      }
       st_chunk[p] = c; st_cnt[p] = FAST ? (f | (f << 16)) : f;
     }
   }
   // FAST: one pass over the regions -- write the complete groups of 8 records of every ring to its chunk, close chunks that are
   // nearly full.  Between two barriers; `finish` also writes the incomplete group (end of the launch).
   const uint32_t rlen = pd.ring_len;
+  // the word of slot s of region p's ring.  Every ring starts at bank 0 and a pass reads the rings of 32 consecutive regions
+  // in 16-byte pieces at fill levels that are multiples of 8, which would touch only every other group of 4 banks: ring p is
+  // rotated by 4 (p & 7) words so that they touch all of them
+  auto ring_word = [&](const uint32_t p, const uint32_t s) -> uint32_t { return p * rlen + ((s + 4u * (p & 7u)) & (rlen - 1)); };
   auto flush_rings = [&](const bool finish) {
     for(uint32_t p = tid; p < pd.P; p += NTH) {
       const uint32_t v = st_cnt[p];
@@ -163,18 +190,17 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
       const uint32_t c = st_chunk[p];
       if(c == NO_CHUNK) continue;
       uint32_t* dst = reinterpret_cast<uint32_t*>(pd.pool + (size_t)c * CHUNK_BYTES);
-      const uint32_t* rg = ring + p * rlen;
-      while((fl & 7u) && fl < cnt) { dst[fl] = rg[fl & (rlen - 1)]; ++fl; }          // (only after a launch that ended inside a group)
+      while((fl & 7u) && fl < cnt) { dst[fl] = ring[ring_word(p, fl)]; ++fl; }          // (only after a launch that ended inside a group)
       while(cnt - fl >= 8u) {
-        const uint4 x0 = *reinterpret_cast<const uint4*>(rg + (fl & (rlen - 1))), x1 = *reinterpret_cast<const uint4*>(rg + (fl & (rlen - 1)) + 4);
+        const uint4 x0 = *reinterpret_cast<const uint4*>(ring + ring_word(p, fl)), x1 = *reinterpret_cast<const uint4*>(ring + ring_word(p, fl + 4));
         *reinterpret_cast<uint4*>(dst + fl) = x0; *reinterpret_cast<uint4*>(dst + fl + 4) = x1;
         fl += 8;
       }
       const bool close = cnt + min(rlen, pd.margin) > pd.chunk_recs;
-      if(close || finish) for(; fl < cnt; ++fl) dst[fl] = rg[fl & (rlen - 1)];
+      if(close || finish) for(; fl < cnt; ++fl) dst[fl] = ring[ring_word(p, fl)];
       if(close) {
         pd.dir[c] = make_uint2(p, cnt);
-        const uint32_t nc = alloc_chunk(pd, pd.by_owner ? (p >> pd.owner_shift) : blockIdx.x);
+        const uint32_t nc = take_chunk(p);
         st_chunk[p] = nc;
         if(nc == NO_CHUNK) { atomicAdd(&a.T.stats[STAT_POOL_FULL], 1ull); cnt = fl = pd.chunk_recs; }
         else cnt = fl = 0;
@@ -678,7 +704,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
           auto ring_append = [&](const uint32_t p, const uint32_t rec, const int j) {
             const uint32_t v = atomicAdd(&st_cnt[p], 1u);
             const uint32_t slot = v & 0xFFFFu, fl = v >> 16;
-            if(slot - fl < rlen && slot < pd.chunk_recs) ring[p * rlen + (slot & (rlen - 1))] = rec;
+            if(slot - fl < rlen && slot < pd.chunk_recs) ring[ring_word(p, slot)] = rec;
             else if(pd.by_owner) atomicAdd(&a.T.stats[STAT_ROUTE_DROPPED], 1ull);   // sharded send side: another shard's k-mer cannot be spilled here
             else {
               uint64_t key[KW];
@@ -712,6 +738,10 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
 #pragma unroll
               for(int jj = 0; jj < SG; ++jj) if((vm4 >> jj) & 1u) ring_append(P[jj], R[jj], hf + jj);
             }
+            // single-GPU counting: one ring pass per 8 k-mers per thread.  A ring of 32 then takes Poisson(8) records per pass on
+            // top of at most 7 of an incomplete group and overflows in about 1e-6 of the region-passes, into the exact spill list.
+            // The sharded send side cannot spill another shard's k-mer, so it keeps a pass per SG k-mers.
+            if(hf + SG < 8 && !pd.by_owner) continue;
             __syncthreads();
             flush_rings(false);
             __syncthreads();
@@ -780,6 +810,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
   if(MODE == 2) {          // keep the open chunks for the next launch
     if(FAST) { flush_rings(true); __syncthreads(); }
     for(uint32_t p = tid; p < pd.P; p += NTH) { my_chunk[p] = st_chunk[p]; my_fill[p] = min(FAST ? (st_cnt[p] & 0xFFFFu) : st_cnt[p], pd.chunk_recs); }
+    if(own_arena && tid == 0) pd.pool_next[blockIdx.x] = *arena_next;
   }
 
   // ---- statistics: one atomic per counter per CTA (a query leaves them alone) ----
