@@ -521,19 +521,22 @@ int read_stats(jfgpu_engine* e);
 int bloom_draw(jfgpu_engine* e);
 BloomDev bloom_dev(const jfgpu_engine* e);
 
-// The window form of K2 (jf_window.cuh): the default for 32-bit slots and 4-byte records.
-// Processes whole regions in groups, starting at unit `*done` (which must be the first unit of a
-// region), until every unit is inserted or -- with regrow enabled -- a group has reported keys that
-// found no slot.  Regions too large for the group buffer are left to the L2 kernel.
-// Post a copy of the live failure counter behind the work enqueued so far / wait for an earlier one.
-static void watch_post(jfgpu_engine* e, cudaStream_t st, int slot) {
-  cudaMemcpyAsync(e->h_watch + slot, e->stats.as<unsigned long long>() + STAT_FAILED, 8, cudaMemcpyDeviceToHost, st);
-  cudaEventRecord(e->ev_watch[slot], st);
-}
-static bool watch_failed(jfgpu_engine* e, int slot) {
-  cudaEventSynchronize(e->ev_watch[slot]);
-  return e->h_watch[slot] != 0;
-}
+// The failure counter of a drain, looked at one step late (hash_counter::add -> handle_full_ary) so that the device never
+// waits for the host: two steps of failed keys fit the failure list (a step is at most fail_group records), and in a
+// write-only drain so does the one deferred list that runs a step later still (fail_cap, jfgpu_create).
+struct FailWatch {
+  jfgpu_engine* e; cudaStream_t st;
+  unsigned n = 0;                // copies posted since the drain began or the table was rebuilt
+  // Post a copy of the live counter behind the work enqueued so far.  True when the copy of the step before shows failed
+  // keys, or after the last step the copy just posted.
+  bool step(bool last) {
+    const int slot = (int)(n++ & 1);
+    cudaMemcpyAsync(e->h_watch + slot, e->stats.as<unsigned long long>() + STAT_FAILED, 8, cudaMemcpyDeviceToHost, st);
+    cudaEventRecord(e->ev_watch[slot], st);
+    return (n > 1 && seen(slot ^ 1)) || (last && seen(slot));
+  }
+  bool seen(int slot) { cudaEventSynchronize(e->ev_watch[slot]); return e->h_watch[slot] != 0; }
+};
 static cudaEvent_t win_event(jfgpu_engine* e, cudaStream_t st) {
   if(e->wev_used == e->wev.size()) { cudaEvent_t ev; cudaEventCreate(&ev); e->wev.push_back(ev); }
   cudaEvent_t ev = e->wev[e->wev_used++];
@@ -568,277 +571,237 @@ static bool lazy_zero_ok(jfgpu_engine* e) {
   return e->part.P && e->bloom.mode == BLOOM_NONE && window_enabled(e, part_dev(e)) &&
          tri(e->tab.max_reprobe) < ((uint64_t)1 << e->part.region_bits);
 }
-int read_stats(jfgpu_engine* e);
-static int window_drain(jfgpu_engine* e, cudaStream_t st, const PartDev& pd, unsigned n_units, bool careful, unsigned group_units,
-                        unsigned* done, bool* failed) {
+// Insert everything that sits in the record pool (K1b), then the spill list.  One loop over the units (chunks in region
+// order); a step is a group of regions in the window form of K2 (jf_window.cuh), a range of units in the L2 form, or, once
+// the table has been doubled, a range in the rehash form.  With regrow enabled the steps are small enough for the failure
+// list, and the failure counter is watched after each one.
+int part_drain(jfgpu_engine* e, cudaStream_t st) {
   PartState& ps = e->part;
-  *failed = false;
-  const uint32_t wpr_lg = pd.region_bits - WIN_LG;
-  if(!ps.w_rec.p) {
-    ps.w_rec_cap = (uint64_t)64 << 20;                       // records per group (256 MB)
-    ps.w_def_cap = WIN_DEF_CAP;
-    bool ok = ps.w_rec.alloc(ps.w_rec_cap * 4 + 64) == cudaSuccess && ps.w_start.alloc((((size_t)WIN_MAX_G << 11) + 1) * 4) == cudaSuccess &&
-              ps.w_cursor.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_cnt.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_def_n.alloc(16) == cudaSuccess &&
-              ps.w_flag.alloc(PMAX * 4) == cudaSuccess;
-    for(int i = 0; i < 2 && ok; ++i) ok = ps.w_def_pos[i].alloc(ps.w_def_cap * 8) == cudaSuccess && ps.w_def_high[i].alloc(ps.w_def_cap * 4) == cudaSuccess;
-    if(!ok) { cudaGetLastError(); return fail(e, JFGPU_ERR_NOMEM, "device allocation of the window buffers failed"); }
-    CUDA_OK(e, cudaMemsetAsync(ps.w_def_n.p, 0, 16, st));
+  if(!ps.P || !ps.pool.p || !ps.pending) return JFGPU_OK;
+  PartDev pd = part_dev(e);
+  // The form is decided once, for the geometry the records were written with.  A doubling in the middle of the drain does
+  // not change it: it only narrows the key field (hb falls by one, the carried reprobe limit stays), so a 32-bit slot
+  // stays 32-bit.
+  const bool win = window_enabled(e, pd);
+  const int g = e->n_sm * 4;
+  if(!e->ev_d0) { cudaEventCreate(&e->ev_d0); cudaEventCreate(&e->ev_d1); }
+  cudaEventRecord(e->ev_d0, st);
+  close_chunks_kernel<<<g, 256, 0, st>>>(pd, (uint32_t)e->n_sm); JF_LAUNCHED();
+  CUDA_OK(e, cudaMemsetAsync(ps.hist.p, 0, PMAX * 12, st));
+  chunk_hist_kernel<<<g, 256, 0, st>>>(pd, ps.hist.as<uint32_t>(), win ? region_recs(ps) : nullptr); JF_LAUNCHED();
+  chunk_scan_kernel<<<1, 1024, 0, st>>>(pd.P, ps.hist.as<uint32_t>(), ps.start.as<uint32_t>(), ps.cursor.as<uint32_t>(), pd.n_units); JF_LAUNCHED();
+  chunk_scatter_kernel<<<g, 256, 0, st>>>(pd, ps.cursor.as<uint32_t>(), ps.order.as<uint32_t>()); JF_LAUNCHED();
+  CUDA_OK(e, cudaMemsetAsync(ps.unit_cursor.p, 0, 8, st));
+  // geometry the records were written with (a regrow in the middle changes e->tab)
+  const TableDev T0 = table_dev(e, e->tab);
+  const bool careful = e->p.allow_regrow != 0 || e->spill_fn != nullptr;
+  unsigned int n_units = 0xFFFFFFFFu;           // (not read when one range of the L2 form takes them all)
+  if(careful || win) {
+    CUDA_OK(e, cudaMemcpyAsync(&n_units, pd.n_units, 4, cudaMemcpyDeviceToHost, st));
+    CUDA_OK(e, cudaStreamSynchronize(st));
+    n_units = std::min(n_units, ps.n_chunks);
   }
-  const TableDev T = table_dev(e, e->tab);
-  // Write-only drain (the table was zeroed lazily; only the windows K1 inserted into are in memory): win_insert2 loads no
-  // other window, win_zero writes the other windows that get no record, and `materialized` follows group by group.  The
-  // deferred records of a group are applied after the next group's windows are written (win_insert2 would overwrite what
-  // they put there), the last group's once the rest of the table is zeroed.  Deferred list of group i: i & 1.
-  bool zero = e->tab.materialized == 0;
-  int def_wait = -1;                                         // deferred list not applied yet
-  auto run_deferred = [&](int set) {
-    WinDev wd;
-    memset(&wd, 0, sizeof(wd));
-    wd.def_pos = ps.w_def_pos[set].as<uint64_t>(); wd.def_high = ps.w_def_high[set].as<uint32_t>();
-    wd.def_n = ps.w_def_n.as<unsigned long long>() + set; wd.def_cap = ps.w_def_cap;
-    if(e->kw == 1) win_deferred_kernel<1><<<e->n_sm * 2, 256, 0, st>>>(T, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
-    else           win_deferred_kernel<2><<<e->n_sm * 2, 256, 0, st>>>(T, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
-    JF_LAUNCHED();
-    cudaMemsetAsync(wd.def_n, 0, 8, st);
-  };
-  auto end_zero = [&]() -> int {                             // the rest of the table in memory, then the waiting deferred records
-    if(!zero) return JFGPU_OK;
-    const int rc = table_materialize(e, e->tab, st);
-    if(rc) return rc;
-    if(def_wait >= 0) run_deferred(def_wait);
-    def_wait = -1; zero = false;
-    return JFGPU_OK;
-  };
-  // the groups' overflow flags (k2_mode 3: set from the start, so that every group takes the exact placement)
-  CUDA_OK(e, cudaMemsetAsync(ps.w_flag.p, e->p.k2_mode == 3 ? 1 : 0, PMAX * 4, st));
-  // first unit and records of every region (chunk_scan_kernel, chunk_hist_kernel), on the host
+  const unsigned group = careful ? (unsigned)std::max<uint64_t>(1, e->fail_group / pd.chunk_recs) : 0xFFFFFFFFu;
+
+  // window form: the first unit and the records of every region (chunk_scan_kernel, chunk_hist_kernel), on the host
+  const uint32_t wpr_lg = win ? pd.region_bits - WIN_LG : 0;
+  const uint64_t wpr = (uint64_t)1 << wpr_lg;
+  const size_t scatter_smem = ((size_t)4 * wpr + (size_t)WIN_ST_UNITS * pd.chunk_recs) * 4;
   std::vector<uint32_t> start(pd.P + 1);
   std::vector<unsigned long long> recs(pd.P);
-  CUDA_OK(e, cudaMemcpyAsync(start.data(), ps.start.p, (size_t)pd.P * 4, cudaMemcpyDeviceToHost, st));
-  CUDA_OK(e, cudaMemcpyAsync(recs.data(), region_recs(ps), (size_t)pd.P * 8, cudaMemcpyDeviceToHost, st));
-  CUDA_OK(e, cudaStreamSynchronize(st));
-  start[pd.P] = n_units;
-  for(uint32_t r = 0; r < pd.P; ++r) start[r] = std::min(start[r], n_units);
-  uint32_t r0 = 0;
-  while(r0 < pd.P && start[r0] < *done) ++r0;
-  const size_t scatter_smem = ((size_t)4 * ((size_t)1 << wpr_lg) + (size_t)WIN_ST_UNITS * pd.chunk_recs) * 4;
-  cudaFuncSetAttribute(win_scatter_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scatter_smem);
-  cudaFuncSetAttribute(win_scatter_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scatter_smem);
+  auto win_begin = [&]() -> int {
+    if(!ps.w_rec.p) {
+      ps.w_rec_cap = (uint64_t)64 << 20;                       // records per group (256 MB)
+      ps.w_def_cap = WIN_DEF_CAP;
+      bool ok = ps.w_rec.alloc(ps.w_rec_cap * 4 + 64) == cudaSuccess && ps.w_start.alloc((((size_t)WIN_MAX_G << 11) + 1) * 4) == cudaSuccess &&
+                ps.w_cursor.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_cnt.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_def_n.alloc(16) == cudaSuccess &&
+                ps.w_flag.alloc(PMAX * 4) == cudaSuccess;
+      for(int i = 0; i < 2 && ok; ++i) ok = ps.w_def_pos[i].alloc(ps.w_def_cap * 8) == cudaSuccess && ps.w_def_high[i].alloc(ps.w_def_cap * 4) == cudaSuccess;
+      if(!ok) { cudaGetLastError(); return fail(e, JFGPU_ERR_NOMEM, "device allocation of the window buffers failed"); }
+      CUDA_OK(e, cudaMemsetAsync(ps.w_def_n.p, 0, 16, st));
+    }
+    // the groups' overflow flags (k2_mode 3: set from the start, so that every group takes the exact placement)
+    CUDA_OK(e, cudaMemsetAsync(ps.w_flag.p, e->p.k2_mode == 3 ? 1 : 0, PMAX * 4, st));
+    CUDA_OK(e, cudaMemcpyAsync(start.data(), ps.start.p, (size_t)pd.P * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_OK(e, cudaMemcpyAsync(recs.data(), region_recs(ps), (size_t)pd.P * 8, cudaMemcpyDeviceToHost, st));
+    CUDA_OK(e, cudaStreamSynchronize(st));
+    start[pd.P] = n_units;
+    for(uint32_t r = 0; r < pd.P; ++r) start[r] = std::min(start[r], n_units);
+    cudaFuncSetAttribute(win_scatter_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scatter_smem);
+    cudaFuncSetAttribute(win_scatter_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scatter_smem);
+    return JFGPU_OK;
+  };
+  int rc = win ? win_begin() : JFGPU_OK;
   // Bucket capacity of a group: m = the largest mean of records per window over its regions.  A window's count is about
   // Poisson(m) for hashed input; m + 6 sqrt(m) + 16 leaves a window of iid input a chance of order 1e-9 to overflow, i.e.
   // a fallback to the exact placement about once in two thousand steps of configs[1] (half a million windows).  k2_mode 4
   // leaves no slack, so nearly every group overflows.  Regions join a group while its buckets fit the group buffer, and
   // so does its exact layout: the group's records (at most m per window on average) plus up to 3 padding records per
   // window, since every run starts on a 16-byte boundary.
-  const uint64_t wpr = (uint64_t)1 << wpr_lg;
   auto bucket_cap = [&](uint64_t m) -> uint64_t {
     const uint64_t c = e->p.k2_mode == 4 ? m : m + (uint64_t)std::ceil(6.0 * std::sqrt((double)m)) + 16;
     return (c + 3) & ~(uint64_t)3;
   };
-  uint32_t gi = 0, ng = 0;
-  while(r0 < pd.P && *done < n_units) {
+  // Write-only drain (the table was zeroed lazily; only the windows K1 inserted into are in memory): win_insert2 loads no
+  // other window, win_zero writes the other windows that get no record, and `materialized` follows group by group.  The
+  // deferred records of a group are applied after the next group's windows are written (win_insert2 would overwrite what
+  // they put there), the last group's once the rest of the table is zeroed.  Deferred list of group i: i & 1.
+  bool zero = win && e->tab.materialized == 0;
+  int def_wait = -1;                                         // deferred list not applied yet
+  auto run_deferred = [&](int set) {
     WinDev wd;
     memset(&wd, 0, sizeof(wd));
-    uint32_t G = 0, stiles = 0;
-    uint64_t m = 0, cap = 0;
-    while(r0 + G < pd.P && G < WIN_MAX_G) {
-      const uint32_t nu = start[r0 + G + 1] - start[r0 + G];
-      if(careful && start[r0 + G + 1] - start[r0] > group_units) break;
-      const uint64_t m2 = std::max<uint64_t>(m, (recs[r0 + G] + wpr - 1) / wpr), cap2 = bucket_cap(m2);
-      if((G + 1) * wpr * std::max(cap2, m2 + 3) > ps.w_rec_cap) break;
-      m = m2; cap = cap2;
-      wd.stile_first[G] = stiles; wd.unit_first[G] = start[r0 + G];
-      stiles += (nu + WIN_ST_UNITS - 1) / WIN_ST_UNITS;
-      ++G;
-    }
-    if(G == 0) {
-      // a single region holds more records than the group buffer (heavily repeated k-mers): L2 kernel for it, whose probes
-      // read the slots of the next region too
-      int rc = end_zero();
-      if(rc) return rc;
-      const unsigned upto = start[r0 + 1];
-      cudaMemsetAsync(ps.unit_cursor.p, 0, 8, st);
-      if(e->kw == 1) insert_chunks32_kernel<1><<<e->n_sm * 2, 768, 0, st>>>(T, pd, ps.order.as<uint32_t>(), ps.unit_cursor.as<unsigned int>(), *done, upto, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
-      else           insert_chunks32_kernel<2><<<e->n_sm * 2, 768, 0, st>>>(T, pd, ps.order.as<uint32_t>(), ps.unit_cursor.as<unsigned int>(), *done, upto, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
-      JF_LAUNCHED();
-      *done = upto; r0 += 1;
-    } else {
-      wd.stile_first[G] = stiles; wd.unit_first[G] = start[r0 + G];
-      wd.g0 = r0; wd.G = G; wd.wpr_lg = wpr_lg; wd.n_tiles = stiles; wd.cap = (uint32_t)cap;
-      wd.overflow = ps.w_flag.as<uint32_t>() + e->wev_used / 4;      // (flag j: the drain's j-th group with records, resolve_win_events)
-      wd.wstart = ps.w_start.as<uint32_t>(); wd.wcursor = ps.w_cursor.as<uint32_t>(); wd.wcnt = ps.w_cnt.as<uint32_t>();
-      wd.wrec = ps.w_rec.as<uint32_t>(); wd.wrec_cap = ps.w_rec_cap;
-      const int set = zero ? (int)(ng & 1) : 0;
-      wd.def_pos = ps.w_def_pos[set].as<uint64_t>(); wd.def_high = ps.w_def_high[set].as<uint32_t>();
-      wd.def_n = ps.w_def_n.as<unsigned long long>() + set; wd.def_cap = ps.w_def_cap;
-      wd.lazy_win = zero ? e->tab.win_state.as<uint32_t>() : nullptr;
-      const uint32_t hb = e->tab.fbits - e->tab.rbits;
-      // the deferred records, once every slot they can reach holds its value in memory
-      auto settle = [&]() {
-        if(!zero) { if(stiles) run_deferred(set); return; }
-        e->tab.materialized = (uint64_t)(r0 + G) << pd.region_bits;
-        if(def_wait >= 0) run_deferred(def_wait);
-        def_wait = stiles ? set : -1;
-      };
-      ++ng;
-      if(stiles) {
-        CUDA_OK(e, cudaMemsetAsync(ps.w_cursor.p, 0, ((size_t)G << wpr_lg) * 4, st));
-        win_event(e, st);
-        win_scatter_kernel<true><<<stiles, WIN_ST_NTH, scatter_smem, st>>>(pd, wd, ps.order.as<uint32_t>(), hb); JF_LAUNCHED();
-        win_scan_kernel<<<1, 1024, 0, st>>>(wd, T.stats); JF_LAUNCHED();
-        win_event(e, st);
-        win_scatter_kernel<false><<<std::min<uint32_t>(stiles, e->n_sm * 2), WIN_ST_NTH, scatter_smem, st>>>(pd, wd, ps.order.as<uint32_t>(), hb);
-        JF_LAUNCHED();
-        win_event(e, st);
-        if(e->kw == 1) {
-          cudaFuncSetAttribute(win_insert2_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WIN2_SMEM);
-          win_insert2_kernel<1><<<e->n_sm, WIN2_NTH, WIN2_SMEM, st>>>(T, pd, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes); JF_LAUNCHED();
-        } else {
-          cudaFuncSetAttribute(win_insert2_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WIN2_SMEM);
-          win_insert2_kernel<2><<<e->n_sm, WIN2_NTH, WIN2_SMEM, st>>>(T, pd, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes); JF_LAUNCHED();
-        }
-        if(zero) {
-          win_zero_kernel<<<e->n_sm * 4, 256, 0, st>>>(e->tab.slots.as<uint32_t>(), wd.lazy_win, wd.wcnt, (uint64_t)r0 << wpr_lg, G << wpr_lg);
-          JF_LAUNCHED();
-        }
-        settle();
-        win_event(e, st);
-      } else {
-        if(zero) {
-          win_zero_kernel<<<e->n_sm * 4, 256, 0, st>>>(e->tab.slots.as<uint32_t>(), wd.lazy_win, nullptr, (uint64_t)r0 << wpr_lg, G << wpr_lg);
-          JF_LAUNCHED();
-        }
-        settle();
-      }
-      *done = start[r0 + G]; r0 += G;
-    }
-    if(careful) {
-      // the failure counter is looked at one group late, so that the device never waits for the host: two groups of
-      // failed keys fit the failure list (group = fail_group records), and in a write-only drain the one deferred list that
-      // runs a group later still (fail_cap, jfgpu_create)
-      watch_post(e, st, (int)(gi & 1));
-      if(gi > 0 && watch_failed(e, (int)((gi - 1) & 1))) {
-        // (the old table is collected next: all of it in memory, every deferred record applied)
-        int rc = end_zero();
-        if(rc) return rc;
-        cudaStreamSynchronize(st); *failed = true; return JFGPU_OK;
-      }
-      ++gi;
-    }
-  }
-  if(zero) {
-    int rc = end_zero();
-    if(rc) return rc;
-    if(careful) { watch_post(e, st, (int)(gi & 1)); ++gi; }      // (the last deferred records may have failed)
-  }
-  if(careful && gi > 0 && watch_failed(e, (int)((gi - 1) & 1))) { cudaStreamSynchronize(st); *failed = true; return JFGPU_OK; }
-  CUDA_OK(e, cudaGetLastError());
-  return JFGPU_OK;
-}
-
-// Insert everything that sits in the record pool (K1b), region by region, then the spill list.
-// With regrow enabled the chunks go in groups small enough for the failure list, and the
-// failure counter is checked after each group (hash_counter::add -> handle_full_ary).
-int part_drain(jfgpu_engine* e, cudaStream_t st) {
-  PartState& ps = e->part;
-  if(!ps.P || !ps.pool.p || !ps.pending) return JFGPU_OK;
-  PartDev pd = part_dev(e);
-  const int g = e->n_sm * 4;
-  if(!e->ev_d0) { cudaEventCreate(&e->ev_d0); cudaEventCreate(&e->ev_d1); }
-  cudaEventRecord(e->ev_d0, st);
-  close_chunks_kernel<<<g, 256, 0, st>>>(pd, (uint32_t)e->n_sm); JF_LAUNCHED();
-  CUDA_OK(e, cudaMemsetAsync(ps.hist.p, 0, PMAX * 12, st));
-  chunk_hist_kernel<<<g, 256, 0, st>>>(pd, ps.hist.as<uint32_t>(), window_enabled(e, pd) ? region_recs(ps) : nullptr); JF_LAUNCHED();
-  chunk_scan_kernel<<<1, 1024, 0, st>>>(pd.P, ps.hist.as<uint32_t>(), ps.start.as<uint32_t>(), ps.cursor.as<uint32_t>(), pd.n_units); JF_LAUNCHED();
-  chunk_scatter_kernel<<<g, 256, 0, st>>>(pd, ps.cursor.as<uint32_t>(), ps.order.as<uint32_t>()); JF_LAUNCHED();
-  CUDA_OK(e, cudaMemsetAsync(ps.unit_cursor.p, 0, 8, st));
-  // geometry the records were written with (a regrow in the middle changes e->tab)
-  const TableDev T0 = table_dev(e, e->tab);
-  const unsigned sb0 = e->tab.slot_bits;
-  const bool careful = e->p.allow_regrow != 0 || e->spill_fn != nullptr;
-  unsigned int n_units = 0;
-  if(careful) {
-    CUDA_OK(e, cudaMemcpyAsync(&n_units, pd.n_units, 4, cudaMemcpyDeviceToHost, st));
-    CUDA_OK(e, cudaStreamSynchronize(st));
-    n_units = std::min(n_units, ps.n_chunks);
-  }
-  const unsigned group = careful ? (unsigned)std::max<uint64_t>(1, e->fail_group / pd.chunk_recs) : 0xFFFFFFFFu;
-  int rc = JFGPU_OK;
+    wd.def_pos = ps.w_def_pos[set].as<uint64_t>(); wd.def_high = ps.w_def_high[set].as<uint32_t>();
+    wd.def_n = ps.w_def_n.as<unsigned long long>() + set; wd.def_cap = ps.w_def_cap;
+    if(e->kw == 1) win_deferred_kernel<1><<<e->n_sm * 2, 256, 0, st>>>(T0, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
+    else           win_deferred_kernel<2><<<e->n_sm * 2, 256, 0, st>>>(T0, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
+    JF_LAUNCHED();
+    cudaMemsetAsync(wd.def_n, 0, 8, st);
+  };
+  // the whole table in memory and every deferred record applied: the L2 and rehash forms, the collection of the old table
+  // and the spill list read the slots
+  auto end_zero = [&]() -> int {
+    const int rc2 = table_materialize(e, e->tab, st);
+    if(rc2 || !zero) return rc2;
+    if(def_wait >= 0) run_deferred(def_wait);
+    def_wait = -1; zero = false;
+    return JFGPU_OK;
+  };
   DevBuf old_inv;     // inverse tables of the geometry the records belong to, once the table has been rebuilt
-  unsigned done = 0;
   bool rebuilt = false;
-  if(window_enabled(e, pd)) {
-    if(!careful) {
-      CUDA_OK(e, cudaMemcpyAsync(&n_units, pd.n_units, 4, cudaMemcpyDeviceToHost, st));
-      CUDA_OK(e, cudaStreamSynchronize(st));
-      n_units = std::min(n_units, ps.n_chunks);
-    }
-    bool w_failed = false;
-    rc = window_drain(e, st, pd, n_units, careful, group, &done, &w_failed);
-    if(!rc && w_failed) {        // same as below: keep the old inverse tables, rebuild, the rest goes through the rehash kernel
-      if(old_inv.alloc(e->tab.inv_lut.bytes) != cudaSuccess) { cudaGetLastError(); rc = fail(e, JFGPU_ERR_NOMEM, "device allocation failed"); }
-      else {
-        cudaMemcpyAsync(old_inv.p, e->tab.inv_lut.p, e->tab.inv_lut.bytes, cudaMemcpyDeviceToDevice, e->cs);
-        cudaStreamSynchronize(e->cs);
-        rebuilt = true;
-        rc = regrow(e);
-      }
-    }
-  }
-  if(!rc) rc = table_materialize(e, e->tab, st);         // (the L2 and rehash forms and the spill list read the slots)
-  unsigned gq = 0;
-  if(!rc && !(window_enabled(e, pd) && done >= n_units && !rebuilt))
-  do {
-    const unsigned upto = careful ? (unsigned)std::min<uint64_t>((uint64_t)done + group, n_units) : 0xFFFFFFFFu;
+  // units [done, upto) in the L2 form, or in the rehash form once the table has been rebuilt
+  auto range = [&](unsigned done, unsigned upto) -> int {
+    int rc2 = end_zero();
+    if(rc2) return rc2;
     cudaMemsetAsync(ps.unit_cursor.p, 0, 8, st);
-    TableDev T = table_dev(e, e->tab);
-    if(!rebuilt) {
-      if(e->op == 0 && e->tab.slot_bits == 32 && pd.rec_bytes == 4 && e->p.k2_mode != 2) {
-        // lean 32-bit specialisation: 2 CTAs x 1024 threads per SM
-        if(e->kw == 1) insert_chunks32_kernel<1><<<e->n_sm * 2, 768, 0, st>>>(T, pd, ps.order.as<uint32_t>(), ps.unit_cursor.as<unsigned int>(), done, upto, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
-        else           insert_chunks32_kernel<2><<<e->n_sm * 2, 768, 0, st>>>(T, pd, ps.order.as<uint32_t>(), ps.unit_cursor.as<unsigned int>(), done, upto, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
-        rc = JFGPU_OK;
-      } else
-      rc = dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int {
+    const TableDev T = table_dev(e, e->tab);
+    if(rebuilt) {
+      const size_t smem = (size_t)e->nbytes * 256 * 8 * 2;
+      rc2 = dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int {
+        auto kern = rehash_chunks_kernel<decltype(KW)::value, decltype(SB)::value>;
+        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        kern<<<e->n_sm, 512, smem, st>>>(T, T0, pd, ps.order.as<uint32_t>(), ps.unit_cursor.as<unsigned int>(), done, upto,
+                                        old_inv.as<uint64_t>(), e->tab.lut.as<uint64_t>(), e->nbytes);
+        return JFGPU_OK;
+      });
+    } else if(e->op == 0 && e->tab.slot_bits == 32 && pd.rec_bytes == 4 && e->p.k2_mode != 2) {
+      // lean 32-bit specialisation: 2 CTAs x 1024 threads per SM
+      if(e->kw == 1) insert_chunks32_kernel<1><<<e->n_sm * 2, 768, 0, st>>>(T, pd, ps.order.as<uint32_t>(), ps.unit_cursor.as<unsigned int>(), done, upto, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
+      else           insert_chunks32_kernel<2><<<e->n_sm * 2, 768, 0, st>>>(T, pd, ps.order.as<uint32_t>(), ps.unit_cursor.as<unsigned int>(), done, upto, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
+    } else
+      rc2 = dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int {
         insert_chunks_kernel<decltype(KW)::value, decltype(SB)::value><<<e->n_sm * 2, 512, 0, st>>>(
             T, pd, ps.order.as<uint32_t>(), ps.unit_cursor.as<unsigned int>(), done, upto, e->tab.inv_lut.as<uint64_t>(), e->nbytes);
         return JFGPU_OK;
       });
+    if(!rc2) JF_LAUNCHED();
+    return rc2;
+  };
+
+  FailWatch watch{e, st};
+  unsigned done = 0;
+  uint32_t r0 = 0, ng = 0;       // window form: the first region of the next group, the groups so far
+  bool ranged = false;           // a range of the L2 or rehash form has run (they run at least one, an empty one too)
+  while(!rc) {
+    const bool window = win && !rebuilt;
+    if(done >= n_units && (window || ranged)) break;
+    unsigned upto = 0;
+    if(!window) {
+      upto = (unsigned)std::min<uint64_t>((uint64_t)done + group, n_units);
+      rc = range(done, upto);
+      ranged = true;
     } else {
-      const size_t smem = (size_t)e->nbytes * 256 * 8 * 2;
-      rc = dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int {
-        auto kern = rehash_chunks_kernel<decltype(KW)::value, decltype(SB)::value>;
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        kern<<<e->n_sm, 512, smem, st>>>(T, T0, pd, ps.order.as<uint32_t>(), ps.unit_cursor.as<unsigned int>(), done, upto,
-                                            old_inv.as<uint64_t>(), e->tab.lut.as<uint64_t>(), e->nbytes);
-        return JFGPU_OK;
-      });
+      WinDev wd;
+      memset(&wd, 0, sizeof(wd));
+      uint32_t G = 0, stiles = 0;
+      uint64_t m = 0, cap = 0;
+      while(r0 + G < pd.P && G < WIN_MAX_G) {
+        const uint32_t nu = start[r0 + G + 1] - start[r0 + G];
+        if(careful && start[r0 + G + 1] - start[r0] > group) break;
+        const uint64_t m2 = std::max<uint64_t>(m, (recs[r0 + G] + wpr - 1) / wpr), cap2 = bucket_cap(m2);
+        if((G + 1) * wpr * std::max(cap2, m2 + 3) > ps.w_rec_cap) break;
+        m = m2; cap = cap2;
+        wd.stile_first[G] = stiles; wd.unit_first[G] = start[r0 + G];
+        stiles += (nu + WIN_ST_UNITS - 1) / WIN_ST_UNITS;
+        ++G;
+      }
+      if(G == 0) {
+        // a single region holds more records than the group buffer (heavily repeated k-mers): the L2 form for it, whose
+        // probes read the slots of the next region too
+        upto = start[r0 + 1]; r0 += 1;
+        rc = range(done, upto);
+      } else {
+        wd.stile_first[G] = stiles; wd.unit_first[G] = start[r0 + G];
+        wd.g0 = r0; wd.G = G; wd.wpr_lg = wpr_lg; wd.n_tiles = stiles; wd.cap = (uint32_t)cap;
+        wd.overflow = ps.w_flag.as<uint32_t>() + e->wev_used / 4;      // (flag j: the drain's j-th group with records, resolve_win_events)
+        wd.wstart = ps.w_start.as<uint32_t>(); wd.wcursor = ps.w_cursor.as<uint32_t>(); wd.wcnt = ps.w_cnt.as<uint32_t>();
+        wd.wrec = ps.w_rec.as<uint32_t>(); wd.wrec_cap = ps.w_rec_cap;
+        const int set = zero ? (int)(ng & 1) : 0;
+        wd.def_pos = ps.w_def_pos[set].as<uint64_t>(); wd.def_high = ps.w_def_high[set].as<uint32_t>();
+        wd.def_n = ps.w_def_n.as<unsigned long long>() + set; wd.def_cap = ps.w_def_cap;
+        wd.lazy_win = zero ? e->tab.win_state.as<uint32_t>() : nullptr;
+        const uint32_t hb = e->tab.fbits - e->tab.rbits;
+        // the deferred records, once every slot they can reach holds its value in memory
+        auto settle = [&]() {
+          if(!zero) { if(stiles) run_deferred(set); return; }
+          e->tab.materialized = (uint64_t)(r0 + G) << pd.region_bits;
+          if(def_wait >= 0) run_deferred(def_wait);
+          def_wait = stiles ? set : -1;
+        };
+        ++ng;
+        if(stiles) {
+          CUDA_OK(e, cudaMemsetAsync(ps.w_cursor.p, 0, ((size_t)G << wpr_lg) * 4, st));
+          win_event(e, st);
+          win_scatter_kernel<true><<<stiles, WIN_ST_NTH, scatter_smem, st>>>(pd, wd, ps.order.as<uint32_t>(), hb); JF_LAUNCHED();
+          win_scan_kernel<<<1, 1024, 0, st>>>(wd, T0.stats); JF_LAUNCHED();
+          win_event(e, st);
+          win_scatter_kernel<false><<<std::min<uint32_t>(stiles, e->n_sm * 2), WIN_ST_NTH, scatter_smem, st>>>(pd, wd, ps.order.as<uint32_t>(), hb);
+          JF_LAUNCHED();
+          win_event(e, st);
+          if(e->kw == 1) {
+            cudaFuncSetAttribute(win_insert2_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WIN2_SMEM);
+            win_insert2_kernel<1><<<e->n_sm, WIN2_NTH, WIN2_SMEM, st>>>(T0, pd, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes); JF_LAUNCHED();
+          } else {
+            cudaFuncSetAttribute(win_insert2_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WIN2_SMEM);
+            win_insert2_kernel<2><<<e->n_sm, WIN2_NTH, WIN2_SMEM, st>>>(T0, pd, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes); JF_LAUNCHED();
+          }
+          if(zero) {
+            win_zero_kernel<<<e->n_sm * 4, 256, 0, st>>>(e->tab.slots.as<uint32_t>(), wd.lazy_win, wd.wcnt, (uint64_t)r0 << wpr_lg, G << wpr_lg);
+            JF_LAUNCHED();
+          }
+          settle();
+          win_event(e, st);
+        } else {
+          if(zero) {
+            win_zero_kernel<<<e->n_sm * 4, 256, 0, st>>>(e->tab.slots.as<uint32_t>(), wd.lazy_win, nullptr, (uint64_t)r0 << wpr_lg, G << wpr_lg);
+            JF_LAUNCHED();
+          }
+          settle();
+        }
+        upto = start[r0 + G]; r0 += G;
+      }
     }
     if(rc) break;
-    JF_LAUNCHED();
-    if(!careful) break;
     done = upto;
-    // the failure counter is read one group late (two groups of failed keys fit the failure list), so the device
-    // does not idle while the host looks at it; the last group is checked right away
-    watch_post(e, st, (int)(gq & 1));
+    if(!careful) continue;
     const bool last = done >= n_units;
-    bool failed_now = gq > 0 && watch_failed(e, (int)((gq - 1) & 1));
-    if(!failed_now && last) failed_now = watch_failed(e, (int)(gq & 1));
-    ++gq;
-    if(failed_now) {
-      cudaStreamSynchronize(st);
-      gq = 0;                    // the groups launched so far are complete: start the look-behind afresh
-      if(!rebuilt) {            // keep a copy of the inverse tables the pending records were written against
-        if(old_inv.alloc(e->tab.inv_lut.bytes) != cudaSuccess) { cudaGetLastError(); rc = fail(e, JFGPU_ERR_NOMEM, "device allocation failed"); break; }
-        cudaMemcpyAsync(old_inv.p, e->tab.inv_lut.p, e->tab.inv_lut.bytes, cudaMemcpyDeviceToDevice, e->cs);
-        cudaStreamSynchronize(e->cs);
-        rebuilt = true;
-      }
-      rc = regrow(e);
-      if(rc) break;
+    if(last) { rc = end_zero(); if(rc) break; }      // (the last deferred records may fail too: the last copy follows them)
+    if(!watch.step(last)) continue;
+    // keys found no slot: the old table is collected next, all of it in memory with every deferred record applied; a copy
+    // of the inverse tables the pending records were written against is kept, the rest goes through the rehash form
+    rc = end_zero();
+    if(rc) break;
+    cudaStreamSynchronize(st);
+    watch.n = 0;                 // the steps launched so far are complete: start the look-behind afresh
+    if(!rebuilt) {
+      if(old_inv.alloc(e->tab.inv_lut.bytes) != cudaSuccess) { cudaGetLastError(); rc = fail(e, JFGPU_ERR_NOMEM, "device allocation failed"); break; }
+      cudaMemcpyAsync(old_inv.p, e->tab.inv_lut.p, e->tab.inv_lut.bytes, cudaMemcpyDeviceToDevice, e->cs);
+      cudaStreamSynchronize(e->cs);
+      rebuilt = true;
     }
-  } while(done < n_units);
-  (void)sb0;
+    rc = regrow(e);
+  }
+  if(!rc) rc = end_zero();
   if(!rc) {
     // the spilled keys carry full keys: plain insertion into whatever the table is now
     TableDev T = table_dev(e, e->tab);
@@ -865,13 +828,34 @@ int part_drain(jfgpu_engine* e, cudaStream_t st) {
   return JFGPU_OK;
 }
 
+// records a closed chunk of the pool holds at least
+uint64_t chunk_usable(const PartState& ps) { return CHUNK_BYTES / ps.rec_bytes - ps.margin; }
+// chunks of one arena that `per_cta` records may take: the ones they fill, plus those the roll-over passes may leave nearly
+// empty
+uint64_t chunks_for(const PartState& ps, uint64_t per_cta) { return per_cta / chunk_usable(ps) + 2; }
+
+// Reserve `need` chunks of every arena for one launch that writes records into the pool (ps.bound_chunks is a host-side
+// upper bound of the chunks in use in any one arena); drain first when the bound says an arena could fill up.  When that
+// drain doubled the table and the new one is not filled region by region (ps.P == 0), nothing is reserved: the caller
+// inserts directly.
+int part_reserve(jfgpu_engine* e, cudaStream_t st, uint64_t need, const char* too_small) {
+  PartState& ps = e->part;
+  if(ps.bound_chunks + need > ps.arena_chunks) {
+    const int rc = part_drain(e, st);
+    if(rc || !ps.P) return rc;
+  }
+  if(ps.bound_chunks + need > ps.arena_chunks) return fail(e, JFGPU_ERR_NOMEM, too_small);
+  ps.bound_chunks += need;
+  ps.pending = true;
+  return JFGPU_OK;
+}
+
 // no more text per launch than an empty arena can take (small pools: tests, tables that leave little memory)
 size_t part_cap_len(const jfgpu_engine* e, size_t len) {
   const PartState& ps = e->part;
   if(!ps.P || !ps.arena_chunks) return len;
-  const uint64_t usable = CHUNK_BYTES / ps.rec_bytes - ps.margin;
   const uint64_t room = ps.arena_chunks > ps.P + 8 ? ps.arena_chunks - ps.P - 8 : 1;
-  const uint64_t tiles_per_cta = std::max<uint64_t>(room * usable / (1024 * 32), 1);
+  const uint64_t tiles_per_cta = std::max<uint64_t>(room * chunk_usable(ps) / (1024 * 32), 1);
   const uint64_t cap = tiles_per_cta * (1024 * 32 - HALO) * (uint64_t)e->n_sm / 2;
   return len > cap ? (size_t)std::max<uint64_t>(cap & ~(uint64_t)15, 16) : len;
 }
@@ -880,40 +864,39 @@ size_t part_cap_len(const jfgpu_engine* e, size_t len) {
 // (a query reads its text as query_from_sequence does, without qualities)
 static uint32_t eff_min_qual(const jfgpu_engine* e) { return e->op == JFGPU_OP_PRIME || e->querying ? 0u : e->p.min_qual; }
 
-// One batch of device-resident text through K0a, K0b, K1 on `stream`.  mode 0: count, 1: route, 3: record exchange, 4: ordered
-// extraction of a query into the buffers e->qb[e->q_cur].
-int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, cudaStream_t stream,
-              int mode, uint64_t* route_keys, unsigned long long* route_counts, uint64_t route_cap, uint64_t n_back = 0) {
+// What K1 does with a batch (the values are what CountArgs.mode carries)
+enum K1Use : uint32_t {
+  K1_COUNT = 0,      // count: into the table, or as region records into the pool
+  K1_ROUTE = 1,      // keys into the caller's buckets by owning shard
+  K1_SEND = 2,       // region records of the GLOBAL table into a bank of the record exchange's send pool
+  K1_QUERY = 4,      // the keys of a query, in input order, into the buffers e->qb[e->q_cur]
+};
+
+// One batch of device-resident text through K0a, K0b, K1 on `stream`.
+int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, cudaStream_t stream, K1Use use, uint64_t n_back = 0,
+              int bank = 0, uint64_t* route_keys = nullptr, unsigned long long* route_counts = nullptr, uint64_t route_cap = 0) {
   if(n == 0) return JFGPU_OK;
   PartState& ps = e->part;
   const bool bc_build = e->bloom.mode == BLOOM_COUNT;
-  const bool part = mode == 0 && ps.P != 0 && !bc_build;
+  bool part = use == K1_COUNT && ps.P != 0 && !bc_build;
   int rc;
   if(e->bloom.mode != BLOOM_NONE && !e->bloom.drawn && (e->op != JFGPU_OP_PRIME || bc_build)) { rc = bloom_draw(e); if(rc) return rc; }
   if(part) {
     rc = part_alloc(e);
     if(rc) return rc;
-    // conservative host-side bound on the use of any one arena: a CTA sees ceil(tiles / CTAs) tiles, one record per
-    // input byte at most, plus the chunks its roll-over passes may leave nearly empty
-    const uint64_t usable = CHUNK_BYTES / ps.rec_bytes - ps.margin;         // records a closed chunk holds at least
+    // a CTA sees ceil(tiles / CTAs) tiles, one record per input byte at most
     const uint64_t tile_b = 1024 * 32 - HALO;
     const uint64_t tiles = (n + tile_b - 1) / tile_b;
-    const uint64_t per_cta = (tiles + e->n_sm - 1) / e->n_sm * tile_b;
-    const uint64_t need = per_cta / usable + 2;
-    if(ps.bound_chunks + need > ps.arena_chunks) {
-      rc = part_drain(e, stream);
-      if(rc) return rc;
-      if(!e->part.P) return run_batch(e, dev, n, n_look, stream, mode, route_keys, route_counts, route_cap, n_back);
-    }
-    if(ps.bound_chunks + need > ps.arena_chunks) return fail(e, JFGPU_ERR_NOMEM, "record pool smaller than one batch");
-    ps.bound_chunks += need;
-    ps.pending = true;
-  } else if(mode == 0 && !bc_build) {            // K1 inserts into the table itself
+    rc = part_reserve(e, stream, chunks_for(ps, (tiles + e->n_sm - 1) / e->n_sm * tile_b), "record pool smaller than one batch");
+    if(rc) return rc;
+    part = ps.P != 0;
+  }
+  if(!part && use == K1_COUNT && !bc_build) {            // K1 inserts into the table itself
     rc = table_materialize(e, e->tab, stream);
     if(rc) return rc;
   }
-  const bool shard_send = mode == 3;            // K1 writes region records of the GLOBAL table into the send pool (bank = route_cap)
-  const bool query = mode == 4;
+  const bool shard_send = use == K1_SEND;
+  const bool query = use == K1_QUERY;
   const uint32_t tile = (part || shard_send ? 1024 : 512) * 32 - HALO;
   const uint64_t n_tiles = (n + tile - 1) / tile;
   rc = ensure_scratch(e, n_tiles);
@@ -938,7 +921,7 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
   a.lut_bytes = e->tab.hash_fast ? 4 * 2048 * 4 : e->nbytes * 256 * 8;
   for(unsigned i = 0; i < 8; ++i) a.prow[i] = e->tab.prow[i];
   a.min_qual = eff_min_qual(e); a.n_back = n_back;
-  a.k = e->k; a.canonical = e->p.canonical; a.nbytes = e->nbytes; a.mode = (uint32_t)(shard_send ? 2 : mode); a.format = (uint32_t)e->format;
+  a.k = e->k; a.canonical = e->p.canonical; a.nbytes = e->nbytes; a.mode = use; a.format = (uint32_t)e->format;
   a.T = table_dev(e, e->tab);
   a.bloom = bloom_dev(e);
   const size_t bloom_smem = a.bloom.mode ? (size_t)e->nbytes * 256 * 8 * 2 : 0;
@@ -948,7 +931,7 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
     a.lut = nullptr; a.lut_bytes = 0; a.hash_fast = 0; memset(&a.bloom, 0, sizeof(a.bloom));
     a.q_keys = e->qb[e->q_cur].keys.as<uint64_t>(); a.q_cnt = e->qb[e->q_cur].cnt.as<uint32_t>(); a.q_tile_cap = tile;
   }
-  PartDev pd = shard_send ? shard_send_dev(e, (int)route_cap) : part_dev(e);
+  PartDev pd = shard_send ? shard_send_dev(e, bank) : part_dev(e);
   auto launch = [&](auto kern, int nth, size_t smem, bool one_per_sm) -> int {
     cudaError_t c = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if(c != cudaSuccess) return fail(e, JFGPU_ERR_CUDA, std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(c));
@@ -971,7 +954,7 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
   if(e->kw == 4) {
     if(query) rc = launch(wide_kernels().extract_query, 512, wide_extract_smem(0), false);
     else if(part || shard_send || a.bloom.mode) rc = fail(e, JFGPU_ERR_ARG, "k > 64 takes neither region records, the record exchange nor a Bloom filter");
-    else if(mode == 1) rc = launch(wide_kernels().extract_route, 512, wide_extract_smem(a.lut_bytes), false);
+    else if(use == K1_ROUTE) rc = launch(wide_kernels().extract_route, 512, wide_extract_smem(a.lut_bytes), false);
     else rc = launch(wide_kernels().extract_count, 512, wide_extract_smem(a.lut_bytes), false);
   } else rc = dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int {
     constexpr int kw = decltype(KW)::value, sb = decltype(SB)::value;
@@ -991,7 +974,7 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
       return launch(extract_kernel<kw, sb, 2, 1024, false>, 1024, count_smem_bytes<1024>(a.lut_bytes, ps.stage_bytes, bloom_smem), true);
     }
     if(query) return launch(extract_kernel<kw, 64, 3, 512, false>, 512, count_smem_bytes<512>(0, 0, 0), false);
-    if(mode == 1) return launch(extract_kernel<kw, sb, 1, 512, false>, 512, count_smem_bytes<512>(a.lut_bytes, 0, bloom_smem), false);
+    if(use == K1_ROUTE) return launch(extract_kernel<kw, sb, 1, 512, false>, 512, count_smem_bytes<512>(a.lut_bytes, 0, bloom_smem), false);
     return launch(extract_kernel<kw, sb, 0, 512, false>, 512, count_smem_bytes<512>(a.lut_bytes, 0, bloom_smem), false);
   });
   if(rc) return rc;
@@ -1145,23 +1128,31 @@ int collect_segment(jfgpu_engine* e, Table& t, SegScratch& s, uint64_t lo, uint6
   return JFGPU_OK;
 }
 
-uint64_t pick_segment(const Table& t) {
-  uint64_t seg = std::min<uint64_t>(t.local_size, (uint64_t)1 << 24);
-  return seg;
+// local positions of a table collected (regrow) or dumped at once
+uint64_t pick_segment(const Table& t) { return std::min<uint64_t>(t.local_size, (uint64_t)1 << 24); }
+
+// While it lives, counts are added (JFGPU_OP_COUNT) whatever operation the counter is in: moving (key, count) pairs into a
+// table, or loading a database, is plain addition.
+struct ForceCount {
+  jfgpu_engine* e; const uint32_t op;
+  explicit ForceCount(jfgpu_engine* e_) : e(e_), op(e_->op) { e->op = JFGPU_OP_COUNT; }
+  ~ForceCount() { e->op = op; }
+};
+
+// Turn to the other failure list (allocated on first use), so that the failures of a re-insertion are kept apart.
+int flip_fail_list(jfgpu_engine* e) {
+  e->fail_cur ^= 1;
+  if(!e->fail_keys[e->fail_cur].p) {
+    CUDA_OK(e, e->fail_keys[e->fail_cur].alloc(e->fail_cap * 8 * e->kw));
+    CUDA_OK(e, e->fail_counts[e->fail_cur].alloc(e->fail_cap * 8));
+  }
+  return JFGPU_OK;
 }
 
 // Move every (key, count) of the current table, plus `n_failed` entries of failure list
 // `old_fail`, into a fresh table of 2^nl global slots hashed with M.
-int rebuild_table_impl(jfgpu_engine* e, unsigned nl, const jfb::gf2_matrix& M, int old_fail, uint64_t n_failed);
 int rebuild_table(jfgpu_engine* e, unsigned nl, const jfb::gf2_matrix& M, int old_fail, uint64_t n_failed) {
-  // moving (key, count) pairs is plain addition whatever operation the counter is in
-  const uint32_t op = e->op;
-  e->op = 0;
-  const int rc = rebuild_table_impl(e, nl, M, old_fail, n_failed);
-  e->op = op;
-  return rc;
-}
-int rebuild_table_impl(jfgpu_engine* e, unsigned nl, const jfb::gf2_matrix& M, int old_fail, uint64_t n_failed) {
+  const ForceCount force_count(e);
   Table nt;
   int rc = table_setup(e, nt, nl, M, e->tab.max_reprobe);
   if(rc) { nt.release(); return rc == JFGPU_ERR_NOMEM ? fail(e, JFGPU_ERR_FULL, "Hash full (" + e->err + ")") : rc; }
@@ -1216,14 +1207,12 @@ int spill_table(jfgpu_engine* e, uint64_t n_failed) {
   CUDA_OK(e, cudaMemsetAsync(st + STAT_FAILED, 0, 8, e->cs));
   CUDA_OK(e, cudaStreamSynchronize(e->cs));
   const int old_fail = e->fail_cur;
-  e->fail_cur ^= 1;                                   // (failures of the re-insertion -- there should be none -- are kept apart)
-  if(!e->fail_keys[e->fail_cur].p) {
-    CUDA_OK(e, e->fail_keys[e->fail_cur].alloc(e->fail_cap * 8 * e->kw));
-    CUDA_OK(e, e->fail_counts[e->fail_cur].alloc(e->fail_cap * 8));
+  rc = flip_fail_list(e);                             // (failures of the re-insertion -- there should be none -- are kept apart)
+  if(rc) return rc;
+  {
+    const ForceCount force_count(e);
+    rc = insert_keys_into(e, e->tab, e->fail_keys[old_fail].as<uint64_t>(), e->fail_counts[old_fail].as<uint64_t>(), n_failed, e->cs);
   }
-  const uint32_t op = e->op; e->op = 0;
-  rc = insert_keys_into(e, e->tab, e->fail_keys[old_fail].as<uint64_t>(), e->fail_counts[old_fail].as<uint64_t>(), n_failed, e->cs);
-  e->op = op;
   if(rc) return rc;
   CUDA_OK(e, cudaStreamSynchronize(e->cs));       // (the keys that had found no slot are counted as inserted now, once)
   e->spills++;
@@ -1247,13 +1236,9 @@ int regrow(jfgpu_engine* e) {
     }
     const unsigned nl = e->tab.lsize + 1;
     jfb::gf2_matrix M = draw_matrix(e, (uint64_t)1 << nl, nl);
-    // switch the failure list so that failures of the re-insertion are kept apart
     const int old_fail = e->fail_cur;
-    e->fail_cur ^= 1;
-    if(!e->fail_keys[e->fail_cur].p) {
-      CUDA_OK(e, e->fail_keys[e->fail_cur].alloc(e->fail_cap * 8 * e->kw));
-      CUDA_OK(e, e->fail_counts[e->fail_cur].alloc(e->fail_cap * 8));
-    }
+    rc = flip_fail_list(e);
+    if(rc) return rc;
     CUDA_OK(e, cudaMemsetAsync(e->stats.as<unsigned long long>() + STAT_FAILED, 0, 8, e->cs));
     rc = rebuild_table(e, nl, M, old_fail, n_failed);
     if(rc == JFGPU_ERR_FULL && e->spill_fn) {          // no memory for the doubled table: dump and zero this one instead
@@ -1429,7 +1414,7 @@ int jfgpu_create(const jfgpu_params* params, jfgpu_handle* out) {
   // side structures
   e->batch_bytes = params->max_batch_bytes ? (size_t)((params->max_batch_bytes + 15) & ~(uint64_t)15) : ((size_t)64 << 20);
   // The failure counter is read one group late: the list holds the failed keys of two groups, and of one deferred list of
-  // a write-only drain (window_drain: a group's deferred records run after the next group; at most WIN_DEF_CAP records and
+  // a write-only drain (part_drain: a group's deferred records run after the next group; at most WIN_DEF_CAP records and
   // at most a group).
   e->fail_group = e->batch_bytes;
   e->fail_cap = 2 * e->fail_group + std::min<uint64_t>(WIN_DEF_CAP, e->fail_group);
@@ -1507,6 +1492,32 @@ static int begin_feed(jfgpu_engine* e, uint32_t flags, int first_byte, cudaStrea
   return JFGPU_OK;
 }
 
+// begin_feed of text in device memory: its first byte is read back to select the format
+static int begin_device_feed(jfgpu_engine* e, uint32_t flags, const void* dev_bytes, size_t n, cudaStream_t st) {
+  int first = -1;
+  if((flags & JFGPU_FILE_BEGIN) && n) {
+    unsigned char b = 0;
+    CUDA_OK(e, cudaMemcpyAsync(&b, dev_bytes, 1, cudaMemcpyDeviceToHost, st));
+    CUDA_OK(e, cudaStreamSynchronize(st));
+    first = b;
+  }
+  return begin_feed(e, flags, first, st);
+}
+
+// One batch of host text through the next staging buffer: copied on the copy stream, run on the compute stream once the
+// copy is done.  The caller has waited for ev_done of that buffer (the previous batch that used it has finished).
+static int run_staged(jfgpu_engine* e, const char* bytes, size_t len, K1Use use) {
+  const int s = e->stage_cur;
+  CUDA_OK(e, cudaMemcpyAsync(e->stage[s].p, bytes, len, cudaMemcpyHostToDevice, e->hs));
+  CUDA_OK(e, cudaEventRecord(e->ev_copied[s], e->hs));
+  CUDA_OK(e, cudaStreamWaitEvent(e->cs, e->ev_copied[s], 0));
+  const int rc = run_batch(e, e->stage[s].as<uint8_t>(), len, len, e->cs, use);
+  if(rc) return rc;
+  CUDA_OK(e, cudaEventRecord(e->ev_done[s], e->cs));
+  e->stage_cur ^= 1;
+  return JFGPU_OK;
+}
+
 static int end_feed(jfgpu_engine* e, uint32_t flags, cudaStream_t st) {
   if(flags & JFGPU_FILE_END) {
     // no k-mer spans two files: mer_overlap_sequence_parser.hpp:111
@@ -1523,14 +1534,7 @@ int jfgpu_feed_device(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_t 
   if(((uintptr_t)dev_bytes & 15) != 0) return fail(e, JFGPU_ERR_ARG, "device text must be 16-byte aligned");
   cudaSetDevice(e->device);
   cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
-  int first = -1;
-  if((flags & JFGPU_FILE_BEGIN) && n) {
-    unsigned char b = 0;
-    CUDA_OK(e, cudaMemcpyAsync(&b, dev_bytes, 1, cudaMemcpyDeviceToHost, st));
-    CUDA_OK(e, cudaStreamSynchronize(st));
-    first = b;
-  }
-  int rc = begin_feed(e, flags, first, st);
+  int rc = begin_device_feed(e, flags, dev_bytes, n, st);
   if(rc) return rc;
   const uint8_t* p = (const uint8_t*)dev_bytes;
   if(e->part.P) { rc = part_alloc(e); if(rc) return rc; }
@@ -1538,7 +1542,7 @@ int jfgpu_feed_device(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_t 
   for(size_t off = 0; off < n; ) {
     size_t len = std::min(e->part.P ? std::max<size_t>(e->batch_bytes, (size_t)512 << 20) : e->batch_bytes, n - off);
     len = part_cap_len(e, len);
-    rc = run_batch(e, p + off, len, n - off, st, 0, nullptr, nullptr, 0, off);
+    rc = run_batch(e, p + off, len, n - off, st, K1_COUNT, off);
     if(rc) return rc;
     off += len;
     if((e->p.allow_regrow || e->spill_fn) && !e->part.P && e->tab.slots.p) {          // the failure list only holds two batches
@@ -1613,22 +1617,16 @@ int jfgpu_feed(jfgpu_handle e, const char* bytes, size_t n, uint32_t flags) {
     size_t len = 0;
     rc = next_batch_len(e, bytes, off, n, part_cap_len(e, std::min(e->batch_bytes, n - off)), qfastq, &len);
     if(rc) return rc;
-    const int s = e->stage_cur;
     // the previous batch that used this staging buffer must be done before it is overwritten
-    CUDA_OK(e, cudaEventSynchronize(e->ev_done[s]));
+    CUDA_OK(e, cudaEventSynchronize(e->ev_done[e->stage_cur]));
     if((e->p.allow_regrow || e->spill_fn) && e->tab.slots.p) {
       // peek at the live failure counter without draining the compute stream
       CUDA_OK(e, cudaMemcpyAsync(e->h_stats + STAT_FAILED, e->stats.as<unsigned long long>() + STAT_FAILED, 8, cudaMemcpyDeviceToHost, e->hs));
       CUDA_OK(e, cudaStreamSynchronize(e->hs));
       if(e->h_stats[STAT_FAILED]) { rc = check_after_batches(e); if(rc) return rc; }
     }
-    CUDA_OK(e, cudaMemcpyAsync(e->stage[s].p, bytes + off, len, cudaMemcpyHostToDevice, e->hs));
-    CUDA_OK(e, cudaEventRecord(e->ev_copied[s], e->hs));
-    CUDA_OK(e, cudaStreamWaitEvent(e->cs, e->ev_copied[s], 0));
-    rc = run_batch(e, e->stage[s].as<uint8_t>(), len, len, e->cs, 0, nullptr, nullptr, 0);
+    rc = run_staged(e, bytes + off, len, K1_COUNT);
     if(rc) return rc;
-    CUDA_OK(e, cudaEventRecord(e->ev_done[s], e->cs));
-    e->stage_cur ^= 1;
     off += len;
   }
   if(qfastq && !(flags & JFGPU_FILE_END)) e->q_lines = 0;       // (the feed was cut behind a complete record)
@@ -1649,19 +1647,12 @@ int jfgpu_extract_route(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_
   if(e->kw == 4 && ((uintptr_t)dev_keys & 15) != 0) return fail(e, JFGPU_ERR_ARG, "route buckets of four-word keys must be 16-byte aligned");
   cudaSetDevice(e->device);
   cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
-  int first = -1;
-  if((flags & JFGPU_FILE_BEGIN) && n) {
-    unsigned char b = 0;
-    CUDA_OK(e, cudaMemcpyAsync(&b, dev_bytes, 1, cudaMemcpyDeviceToHost, st));
-    CUDA_OK(e, cudaStreamSynchronize(st));
-    first = b;
-  }
-  int rc = begin_feed(e, flags, first, st);
+  int rc = begin_device_feed(e, flags, dev_bytes, n, st);
   if(rc) return rc;
   const uint8_t* p = (const uint8_t*)dev_bytes;
   for(size_t off = 0; off < n; ) {
     size_t len = std::min(e->batch_bytes, n - off);
-    rc = run_batch(e, p + off, len, n - off, st, 1, (uint64_t*)dev_keys, (unsigned long long*)dev_counts, capacity, off);
+    rc = run_batch(e, p + off, len, n - off, st, K1_ROUTE, off, 0, (uint64_t*)dev_keys, (unsigned long long*)dev_counts, capacity);
     if(rc) return rc;
     off += len;
   }
@@ -1730,19 +1721,12 @@ int jfgpu_shard_extract(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_
   if(((uintptr_t)dev_bytes & 15) != 0) return fail(e, JFGPU_ERR_ARG, "device text must be 16-byte aligned");
   cudaSetDevice(e->device);
   cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
-  int first = -1;
-  if((flags & JFGPU_FILE_BEGIN) && n) {
-    unsigned char b = 0;
-    CUDA_OK(e, cudaMemcpyAsync(&b, dev_bytes, 1, cudaMemcpyDeviceToHost, st));
-    CUDA_OK(e, cudaStreamSynchronize(st));
-    first = b;
-  }
-  int rc = begin_feed(e, flags, first, st);
+  int rc = begin_device_feed(e, flags, dev_bytes, n, st);
   if(rc) return rc;
   const uint8_t* p = (const uint8_t*)dev_bytes;
   for(size_t off = 0; off < n; ) {
     const size_t len = std::min<size_t>((size_t)512 << 20, n - off);
-    rc = run_batch(e, p + off, len, n - off, st, 3, nullptr, nullptr, bank, off);
+    rc = run_batch(e, p + off, len, n - off, st, K1_SEND, off, (int)bank);
     if(rc) return rc;
     off += len;
   }
@@ -1781,14 +1765,10 @@ int jfgpu_shard_unpack(jfgpu_handle e, const uint64_t* counts, uint32_t self_ban
   uint64_t total = 0;
   for(uint32_t s = 0; s < G; ++s) { if(counts[s] > std::max(e->sh.seg_chunks, e->sh.arena_chunks)) return fail(e, JFGPU_ERR_ARG, "more chunks than a receive segment holds"); total += counts[s]; }
   if(total == 0) return JFGPU_OK;
-  // room in the CTAs' arenas of the local pool (as in run_batch): drain first when the bound says they could fill up
-  const uint64_t usable = CHUNK_BYTES / ps.rec_bytes - ps.margin;
-  const uint64_t per_cta = (total + e->n_sm - 1) / e->n_sm + 1;                  // (chunk j goes to CTA j mod grid)
-  const uint64_t need = per_cta * (CHUNK_BYTES / 4) / usable + 2;
-  if(ps.bound_chunks + need > ps.arena_chunks) { rc = part_drain(e, st); if(rc) return rc; }
-  if(ps.bound_chunks + need > ps.arena_chunks) return fail(e, JFGPU_ERR_NOMEM, "record pool smaller than one exchange round");
-  ps.bound_chunks += need;
-  ps.pending = true;
+  // room in the CTAs' arenas of the local pool for the records of the received chunks (chunk j goes to CTA j mod grid)
+  const uint64_t per_cta = (total + e->n_sm - 1) / e->n_sm + 1;
+  rc = part_reserve(e, st, chunks_for(ps, per_cta * (CHUNK_BYTES / 4)), "record pool smaller than one exchange round");
+  if(rc) return rc;
   rc = table_materialize(e, e->tab, st);      // (restage_kernel inserts the records of a full ring or chunk into the table itself)
   if(rc) return rc;
   RestageArgs ra;
@@ -1824,16 +1804,11 @@ int jfgpu_insert_keys(jfgpu_handle e, const void* dev_keys, uint64_t n, void* st
     // region-by-region mode: turn the keys into records of the pool (K1c); K2 inserts them at the next drain
     rc = part_alloc(e);
     if(rc) return rc;
-    const uint64_t usable = CHUNK_BYTES / ps.rec_bytes - ps.margin;
     const uint64_t per_cta = (n + e->n_sm - 1) / e->n_sm + 1024 * 32;     // keys a CTA of stage_keys_kernel handles at most
-    const uint64_t need = per_cta / usable + 2;
-    if(ps.bound_chunks + need > ps.arena_chunks) { rc = part_drain(e, st); if(rc) return rc; }
-    if(ps.P && ps.bound_chunks + need > ps.arena_chunks) return fail(e, JFGPU_ERR_NOMEM, "record pool smaller than one batch of keys");
+    rc = part_reserve(e, st, chunks_for(ps, per_cta), "record pool smaller than one batch of keys");
+    if(rc) return rc;
   }
   if(ps.P) {
-    const uint64_t usable = CHUNK_BYTES / ps.rec_bytes - ps.margin;
-    ps.bound_chunks += ((n + e->n_sm - 1) / e->n_sm + 1024 * 32) / usable + 2;
-    ps.pending = true;
     PartDev pd = part_dev(e);
     TableDev T = table_dev(e, e->tab);
     const size_t smem = (size_t)e->nbytes * 256 * 8 + PMAX * 8;
@@ -1969,7 +1944,7 @@ int jfgpu_dump(jfgpu_handle e, uint64_t lower, uint64_t upper, uint32_t ocl, jfg
   // it to pinned host memory.
   Table& t = e->tab;
   const unsigned rec = e->nbytes + ocl;
-  const uint64_t seg = std::min<uint64_t>(t.local_size, (uint64_t)1 << 24);
+  const uint64_t seg = pick_segment(t);
   const uint64_t cap = seg + t.margin + 8;                    // records of a segment at most
   const uint32_t max_tiles = (uint32_t)((seg + DUMP_TP - 1) / DUMP_TP);
   DevBuf tile_cnt[2], out[2];
@@ -2099,8 +2074,7 @@ int jfgpu_load_records(jfgpu_handle e, const void* records, size_t nbytes, uint3
     cudaGetLastError();
     rc = fail(e, JFGPU_ERR_NOMEM, "allocation of the load staging buffers failed");
   }
-  const uint32_t op = e->op;
-  e->op = JFGPU_OP_COUNT;                       // the records' counts are added, whatever the counter is doing
+  ForceCount force_count(e);                    // the records' counts are added, whatever the counter is doing
   const uint8_t* src = (const uint8_t*)records;
   if(!rc) memcpy(h[0], src, slice * rec);
   for(uint64_t i = 0, first = 0; first < n_rec && !rc; ++i, first += slice) {
@@ -2119,7 +2093,6 @@ int jfgpu_load_records(jfgpu_handle e, const void* records, size_t nbytes, uint3
     if(first + m < n_rec) memcpy(h[b ^ 1], src + (first + m) * rec, std::min(slice, n_rec - first - m) * rec);
     rc = check_after_batches(e);                // (synchronises; a table that is full is doubled, counts and all)
   }
-  e->op = op;
   cudaStreamSynchronize(e->cs);
   raw.free(); keys.free(); counts.free();
   for(int i = 0; i < 2; ++i) if(h[i]) cudaFreeHost(h[i]);
@@ -2163,16 +2136,10 @@ static int query_impl(jfgpu_engine* e, const char* bytes, size_t n, uint32_t fla
   // text -> k-mers in order -> counts -> where every window's lines start (enqueued on the compute stream)
   auto front = [&](int b, size_t off, size_t len) -> int {
     jfgpu_engine::QueryBufs& q = e->qb[b];
-    const int s = e->stage_cur;
-    CUDA_OK(e, cudaEventSynchronize(e->ev_done[s]));
-    CUDA_OK(e, cudaMemcpyAsync(e->stage[s].p, bytes + off, len, cudaMemcpyHostToDevice, e->hs));
-    CUDA_OK(e, cudaEventRecord(e->ev_copied[s], e->hs));
-    CUDA_OK(e, cudaStreamWaitEvent(e->cs, e->ev_copied[s], 0));
+    CUDA_OK(e, cudaEventSynchronize(e->ev_done[e->stage_cur]));
     e->q_cur = b;
-    int rc2 = run_batch(e, e->stage[s].as<uint8_t>(), len, len, e->cs, 4, nullptr, nullptr, 0);
+    int rc2 = run_staged(e, bytes + off, len, K1_QUERY);
     if(rc2) return rc2;
-    CUDA_OK(e, cudaEventRecord(e->ev_done[s], e->cs));
-    e->stage_cur ^= 1;
     q.n_tiles = (len + TILE - 1) / TILE;
     const int grid = (int)std::min<uint64_t>(q.n_tiles, (uint64_t)e->n_sm * 8);
     auto run = [&](auto kern) -> int {
