@@ -8,6 +8,8 @@
 #include <cstdio>
 #include <cstring>
 #include <string>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../../include/jfgpu.h"
@@ -35,12 +37,67 @@ constexpr uint64_t WIN_DEF_CAP = (uint64_t)16 << 20;   // deferred records per g
 unsigned ceil_log2(uint64_t x) { unsigned l = 0; while(l < 64 && ((uint64_t)1 << l) < x) ++l; return l; }
 unsigned bitsize(uint64_t x) { unsigned b = 0; while(x) { ++b; x >>= 1; } return b ? b : 1; }
 
+// Owners of the engine's CUDA resources.  Each is move-only and empty while it holds nothing; what it holds is released
+// when it is reset, reassigned or destroyed.  An allocation or creation that fails leaves it empty.
 struct DevBuf {
   void* p = nullptr; size_t bytes = 0;
-  cudaError_t alloc(size_t n) { free(); bytes = n; return n ? cudaMalloc(&p, n) : cudaSuccess; }
-  void free() { if(p) cudaFree(p); p = nullptr; bytes = 0; }
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr; o.bytes = 0; }
+  DevBuf& operator=(DevBuf&& o) noexcept { if(this != &o) { reset(); std::swap(p, o.p); std::swap(bytes, o.bytes); } return *this; }
+  ~DevBuf() { reset(); }
+  // (the old buffer is freed first: the old and the new one are never held at once)
+  cudaError_t alloc(size_t n) { reset(); const cudaError_t c = n ? cudaMalloc(&p, n) : cudaSuccess; if(c == cudaSuccess) bytes = n; else p = nullptr; return c; }
+  void reset() { if(p) cudaFree(p); p = nullptr; bytes = 0; }
   template<typename T> T* as() const { return reinterpret_cast<T*>(p); }
 };
+
+template<typename T> struct HostBuf {            // pinned host memory
+  T* p = nullptr;
+  HostBuf() = default;
+  HostBuf(const HostBuf&) = delete;
+  ~HostBuf() { reset(); }
+  cudaError_t alloc(size_t bytes) { reset(); const cudaError_t c = cudaHostAlloc((void**)&p, bytes, cudaHostAllocDefault); if(c) p = nullptr; return c; }
+  void reset() { if(p) cudaFreeHost(p); p = nullptr; }
+  operator T*() const { return p; }
+};
+
+struct Event {
+  cudaEvent_t ev = nullptr;
+  Event() = default;
+  Event(Event&& o) noexcept : ev(o.ev) { o.ev = nullptr; }
+  ~Event() { reset(); }
+  cudaError_t create(unsigned flags) { reset(); const cudaError_t c = cudaEventCreateWithFlags(&ev, flags); if(c) ev = nullptr; return c; }
+  void reset() { if(ev) cudaEventDestroy(ev); ev = nullptr; }
+  operator cudaEvent_t() const { return ev; }
+};
+
+struct Stream {
+  cudaStream_t s = nullptr;
+  Stream() = default;
+  Stream(const Stream&) = delete;
+  ~Stream() { if(s) cudaStreamDestroy(s); }
+  cudaError_t create() { const cudaError_t c = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking); if(c) s = nullptr; return c; }
+  operator cudaStream_t() const { return s; }
+};
+
+// A member of a group for make_all: a buffer of `arg` bytes, or an event created with flags `arg`
+template<typename O> struct Need {
+  O& o; size_t arg;
+  cudaError_t make() const {
+    if constexpr(std::is_same<O, Event>::value) return o.create((unsigned)arg);
+    else return o.alloc(arg);
+  }
+};
+template<typename O> Need<O> need(O& o, size_t arg) { return Need<O>{o, arg}; }
+
+// Make a group of resources all or nothing, in order.  When one fails, every member is reset, the error state is cleared
+// and the error returned; so any one member tells whether the whole group is there.
+template<typename... O> cudaError_t make_all(Need<O>... m) {
+  cudaError_t c = cudaSuccess;
+  (void)(((c = m.make()) == cudaSuccess) && ...);
+  if(c != cudaSuccess) { (m.o.reset(), ...); cudaGetLastError(); }
+  return c;
+}
 
 // byte-indexed tables of a GF(2) matrix: entry [b*256+v] = product with the vector whose
 // byte b equals v (reference column order: bit i selects columns[c-1-i],
@@ -75,7 +132,6 @@ struct Table {
   DevBuf win_state;              // while materialized < local_size: one state per window (jf_kernels.cuh, WIN_LAZY ...)
   uint64_t prow[8] = {0,0,0,0,0,0,0,0}; unsigned n_prow = 0; bool hash_fast = false;
   std::vector<uint64_t> reprobes;
-  void release() { slots.free(); lut.free(); inv_lut.free(); ovf_keys.free(); ovf_vals.free(); lut11.free(); win_state.free(); }
   size_t bytes() const { return (size_t)local_slots * (slot_bits / 8); }
 };
 
@@ -101,7 +157,7 @@ struct ShardState {
   uint64_t arena_chunks = 0, seg_chunks = 0;
   uint8_t* send_pool = nullptr; uint2* send_dir = nullptr; uint8_t* recv_pool = nullptr; uint2* recv_dir = nullptr;
   DevBuf pool_next[2], cta_chunk, cta_fill;
-  unsigned int* h_counts = nullptr;       // pinned
+  HostBuf<unsigned int> h_counts;
 };
 
 struct BloomState {
@@ -111,27 +167,26 @@ struct BloomState {
   jfb::gf2_matrix M1, M2;
   std::vector<uint64_t> cols1, cols2;
   DevBuf bits, locks, lut1, lut2;
-  void release() { bits.free(); locks.free(); lut1.free(); lut2.free(); }
 };
 
 struct jfgpu_engine {
+  Stream cs, hs;                  // (first, so that they are destroyed last)
   jfgpu_params p;
   PartState part;
   ShardState sh;
   BloomState bloom;
   int device = 0;
   unsigned k = 0, kw = 1, nbytes = 0, shard_bits = 0;
-  cudaStream_t cs = nullptr, hs = nullptr;
   int n_sm = 132;
   jfb::glibc_random rng;
   Table tab;
   DevBuf stats, carry[2], fail_keys[2], fail_counts[2];
   uint64_t fail_cap = 0, fail_group = 0;    // failure list entries; records per group of a careful drain
   int carry_cur = 0, fail_cur = 0;
-  unsigned long long* h_stats = nullptr;    // pinned mirror
+  HostBuf<unsigned long long> h_stats;      // mirror of `stats`
   // staging for host feeds
   size_t batch_bytes = 0;
-  DevBuf stage[2]; cudaEvent_t ev_copied[2] = { nullptr, nullptr }, ev_done[2] = { nullptr, nullptr };
+  DevBuf stage[2]; Event ev_copied[2], ev_done[2];
   int stage_cur = 0;
   // per-batch scratch
   DevBuf nlA, nlB, cntA, cntB, tstate; uint64_t scratch_tiles = 0;
@@ -148,29 +203,29 @@ struct jfgpu_engine {
   uint64_t bytes_fed = 0, regrows = 0;
   double count_ms = 0;
   unsigned eff_val_len = 7;
-  cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;
+  Event ev_t0, ev_t1;
   std::string err;
   std::vector<uint64_t> matrix_cols_host;   // for jfgpu_table_info_get
-  std::vector<cudaEvent_t> kev;             // event pairs around count_kernel launches
+  std::vector<Event> kev;                   // event pairs around count_kernel launches
   size_t kev_used = 0;
   double kernel_ms = 0; uint64_t kernel_launches = 0;
-  double drain_ms = 0; cudaEvent_t ev_d0 = nullptr, ev_d1 = nullptr;
+  double drain_ms = 0; Event ev_d0, ev_d1;
   int count_smem = 0;
   // CUDA events around the window kernels of a drain: [4 per group] hist begin, scatter begin, insert begin, insert end
-  std::vector<cudaEvent_t> wev; size_t wev_used = 0;
+  std::vector<Event> wev; size_t wev_used = 0;
   double win_ms[3] = { 0, 0, 0 };
   // failure counter watched one group behind (hash_counter::add -> handle_full_ary), without draining the stream
-  unsigned long long* h_watch = nullptr; cudaEvent_t ev_watch[2] = { nullptr, nullptr };
+  HostBuf<unsigned long long> h_watch; Event ev_watch[2];
   // jfgpu_query: two sets of per-batch buffers (the lines of batch i are copied out while batch i+1 is looked up)
   bool querying = false;
   struct QueryBufs {
     DevBuf keys, vals, cnt, off, out;
-    unsigned long long* h_off = nullptr;    // pinned copy of `off` (entry n_tiles: the batch's total)
-    uint32_t* h_cnt = nullptr;              // pinned copy of `cnt`
+    HostBuf<unsigned long long> h_off;      // copy of `off` (entry n_tiles: the batch's total)
+    HostBuf<uint32_t> h_cnt;                // copy of `cnt`
     uint64_t n_tiles = 0;
-    cudaEvent_t ev_front = nullptr, ev_fmt = nullptr;
+    Event ev_front, ev_fmt;
   } qb[2];
-  uint8_t* q_host[2] = { nullptr, nullptr }; cudaEvent_t ev_qcopy[2] = { nullptr, nullptr };
+  HostBuf<uint8_t> q_host[2]; Event ev_qcopy[2];
   uint64_t q_tiles_cap = 0; int q_cur = 0;
 };
 
@@ -241,13 +296,11 @@ int table_setup(jfgpu_engine* e, Table& t, unsigned lsize, const jfb::gf2_matrix
   t.local_slots = t.local_size + t.margin + 8;
   t.M = M;
   t.Minv = M.pseudo_inverse();
-  if(cudaMalloc(&t.slots.p, t.bytes()) != cudaSuccess) {
+  if(t.slots.alloc(t.bytes()) != cudaSuccess) {
     cudaGetLastError();
-    t.slots.p = nullptr;
     char buf[128]; snprintf(buf, sizeof(buf), "Failed to allocate %zu bytes of device memory", t.bytes());
     return fail(e, JFGPU_ERR_NOMEM, buf);
   }
-  t.slots.bytes = t.bytes();
   // counter-carry side table: one entry per slot whose counter field wrapped; sized with the table
   t.ovf_size = (uint64_t)1 << 20;
   while(t.ovf_size < ((uint64_t)1 << 26) && t.ovf_size * 64 < t.local_size) t.ovf_size <<= 1;
@@ -383,11 +436,8 @@ int ensure_scratch(jfgpu_engine* e, uint64_t n_tiles) {
   if(n_tiles <= e->scratch_tiles) return JFGPU_OK;
   uint64_t want = std::max<uint64_t>(n_tiles, 1024);
   CUDA_OK(e, cudaStreamSynchronize(e->cs));
-  CUDA_OK(e, e->nlA.alloc(want * 8));
-  CUDA_OK(e, e->nlB.alloc(want * 8));
-  CUDA_OK(e, e->cntA.alloc(want * 4));
-  CUDA_OK(e, e->cntB.alloc(want * 4));
-  CUDA_OK(e, e->tstate.alloc(want));
+  e->scratch_tiles = 0;
+  CUDA_OK(e, make_all(need(e->nlA, want * 8), need(e->nlB, want * 8), need(e->cntA, want * 4), need(e->cntB, want * 4), need(e->tstate, want)));
   e->scratch_tiles = want;
   return JFGPU_OK;
 }
@@ -485,13 +535,11 @@ int part_alloc(jfgpu_engine* e) {
   ps.arena_chunks = (uint32_t)std::min<size_t>(want / CHUNK_BYTES / ps.n_arenas, 0xFFFFFFF0u / ps.n_arenas);
   ps.n_chunks = ps.arena_chunks * ps.n_arenas;
   ps.spill_cap = (uint64_t)16 << 20;
-  bool ok = ps.pool.alloc((size_t)ps.n_chunks * CHUNK_BYTES) == cudaSuccess && ps.dir.alloc((size_t)ps.n_chunks * 8) == cudaSuccess &&
-            ps.order.alloc((size_t)ps.n_chunks * 4) == cudaSuccess && ps.pool_next.alloc(((size_t)ps.n_arenas + 2) * 4) == cudaSuccess &&
-            ps.cta_chunk.alloc((size_t)e->n_sm * PMAX * 4) == cudaSuccess && ps.cta_fill.alloc((size_t)e->n_sm * PMAX * 4) == cudaSuccess &&
-            ps.spill_keys.alloc(ps.spill_cap * 8 * e->kw) == cudaSuccess && ps.spill_counts.alloc(ps.spill_cap * 8) == cudaSuccess &&
-            ps.spill_n.alloc(8) == cudaSuccess && ps.hist.alloc(PMAX * 12) == cudaSuccess && ps.start.alloc(PMAX * 4) == cudaSuccess &&
-            ps.cursor.alloc(PMAX * 4) == cudaSuccess && ps.unit_cursor.alloc(8) == cudaSuccess;
-  if(!ok) { cudaGetLastError(); return fail(e, JFGPU_ERR_NOMEM, "device allocation of the record pool failed"); }
+  if(make_all(need(ps.pool, (size_t)ps.n_chunks * CHUNK_BYTES), need(ps.dir, (size_t)ps.n_chunks * 8), need(ps.order, (size_t)ps.n_chunks * 4),
+              need(ps.pool_next, ((size_t)ps.n_arenas + 2) * 4), need(ps.cta_chunk, (size_t)e->n_sm * PMAX * 4),
+              need(ps.cta_fill, (size_t)e->n_sm * PMAX * 4), need(ps.spill_keys, ps.spill_cap * 8 * e->kw), need(ps.spill_counts, ps.spill_cap * 8),
+              need(ps.spill_n, 8), need(ps.hist, PMAX * 12), need(ps.start, PMAX * 4), need(ps.cursor, PMAX * 4), need(ps.unit_cursor, 8)) != cudaSuccess)
+    return fail(e, JFGPU_ERR_NOMEM, "device allocation of the record pool failed");
   CUDA_OK(e, cudaMemsetAsync(ps.pool_next.p, 0, ps.pool_next.bytes, e->cs));
   CUDA_OK(e, cudaMemsetAsync(ps.spill_n.p, 0, 8, e->cs));
   CUDA_OK(e, cudaMemsetAsync(ps.cta_chunk.p, 0xFF, ps.cta_chunk.bytes, e->cs));
@@ -504,16 +552,6 @@ int part_alloc(jfgpu_engine* e) {
 
 // records per region (chunk_hist_kernel), behind the chunk counts in `hist`
 static unsigned long long* region_recs(PartState& ps) { return reinterpret_cast<unsigned long long*>(ps.hist.as<uint32_t>() + PMAX); }
-
-void part_release(jfgpu_engine* e) {
-  PartState& ps = e->part;
-  ps.pool.free(); ps.dir.free(); ps.order.free(); ps.pool_next.free(); ps.cta_chunk.free(); ps.cta_fill.free();
-  ps.spill_keys.free(); ps.spill_counts.free(); ps.spill_n.free(); ps.hist.free(); ps.start.free(); ps.cursor.free(); ps.unit_cursor.free();
-  ps.w_start.free(); ps.w_cursor.free(); ps.w_cnt.free(); ps.w_rec.free(); ps.w_def_n.free(); ps.w_flag.free();
-  for(int i = 0; i < 2; ++i) { ps.w_def_pos[i].free(); ps.w_def_high[i].free(); }
-  ps.w_rec_cap = ps.w_def_cap = 0;
-  ps.n_chunks = 0; ps.arena_chunks = 0; ps.n_arenas = 0; ps.pending = false;
-}
 
 int regrow(jfgpu_engine* e);
 int spill_table(jfgpu_engine* e, uint64_t n_failed);
@@ -537,11 +575,13 @@ struct FailWatch {
   }
   bool seen(int slot) { cudaEventSynchronize(e->ev_watch[slot]); return e->h_watch[slot] != 0; }
 };
-static cudaEvent_t win_event(jfgpu_engine* e, cudaStream_t st) {
-  if(e->wev_used == e->wev.size()) { cudaEvent_t ev; cudaEventCreate(&ev); e->wev.push_back(ev); }
-  cudaEvent_t ev = e->wev[e->wev_used++];
+static cudaError_t win_event(jfgpu_engine* e, cudaStream_t st) {
+  if(e->wev_used == e->wev.size()) e->wev.emplace_back();
+  Event& ev = e->wev[e->wev_used];
+  if(!ev) { const cudaError_t c = make_all(need(ev, cudaEventDefault)); if(c != cudaSuccess) return c; }
   cudaEventRecord(ev, st);
-  return ev;
+  e->wev_used++;
+  return cudaSuccess;
 }
 // Fold the event quadruples of the finished drain into win_ms (the stream must be idle).  Quadruple j belongs to the drain's
 // j-th group with records: bucket pass + scan -> scatter; the exact pass -> hist when that group overflowed a bucket (w_flag[j]),
@@ -584,7 +624,7 @@ int part_drain(jfgpu_engine* e, cudaStream_t st) {
   // stays 32-bit.
   const bool win = window_enabled(e, pd);
   const int g = e->n_sm * 4;
-  if(!e->ev_d0) { cudaEventCreate(&e->ev_d0); cudaEventCreate(&e->ev_d1); }
+  if(!e->ev_d0) CUDA_OK(e, make_all(need(e->ev_d0, cudaEventDefault), need(e->ev_d1, cudaEventDefault)));
   cudaEventRecord(e->ev_d0, st);
   close_chunks_kernel<<<g, 256, 0, st>>>(pd, (uint32_t)e->n_sm); JF_LAUNCHED();
   CUDA_OK(e, cudaMemsetAsync(ps.hist.p, 0, PMAX * 12, st));
@@ -613,11 +653,11 @@ int part_drain(jfgpu_engine* e, cudaStream_t st) {
     if(!ps.w_rec.p) {
       ps.w_rec_cap = (uint64_t)64 << 20;                       // records per group (256 MB)
       ps.w_def_cap = WIN_DEF_CAP;
-      bool ok = ps.w_rec.alloc(ps.w_rec_cap * 4 + 64) == cudaSuccess && ps.w_start.alloc((((size_t)WIN_MAX_G << 11) + 1) * 4) == cudaSuccess &&
-                ps.w_cursor.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_cnt.alloc(((size_t)WIN_MAX_G << 11) * 4) == cudaSuccess && ps.w_def_n.alloc(16) == cudaSuccess &&
-                ps.w_flag.alloc(PMAX * 4) == cudaSuccess;
-      for(int i = 0; i < 2 && ok; ++i) ok = ps.w_def_pos[i].alloc(ps.w_def_cap * 8) == cudaSuccess && ps.w_def_high[i].alloc(ps.w_def_cap * 4) == cudaSuccess;
-      if(!ok) { cudaGetLastError(); return fail(e, JFGPU_ERR_NOMEM, "device allocation of the window buffers failed"); }
+      if(make_all(need(ps.w_rec, ps.w_rec_cap * 4 + 64), need(ps.w_start, (((size_t)WIN_MAX_G << 11) + 1) * 4), need(ps.w_cursor, ((size_t)WIN_MAX_G << 11) * 4),
+                  need(ps.w_cnt, ((size_t)WIN_MAX_G << 11) * 4), need(ps.w_def_n, 16), need(ps.w_flag, PMAX * 4),
+                  need(ps.w_def_pos[0], ps.w_def_cap * 8), need(ps.w_def_high[0], ps.w_def_cap * 4),
+                  need(ps.w_def_pos[1], ps.w_def_cap * 8), need(ps.w_def_high[1], ps.w_def_cap * 4)) != cudaSuccess)
+        return fail(e, JFGPU_ERR_NOMEM, "device allocation of the window buffers failed");
       CUDA_OK(e, cudaMemsetAsync(ps.w_def_n.p, 0, 16, st));
     }
     // the groups' overflow flags (k2_mode 3: set from the start, so that every group takes the exact placement)
@@ -751,13 +791,13 @@ int part_drain(jfgpu_engine* e, cudaStream_t st) {
         ++ng;
         if(stiles) {
           CUDA_OK(e, cudaMemsetAsync(ps.w_cursor.p, 0, ((size_t)G << wpr_lg) * 4, st));
-          win_event(e, st);
+          CUDA_OK(e, win_event(e, st));
           win_scatter_kernel<true><<<stiles, WIN_ST_NTH, scatter_smem, st>>>(pd, wd, ps.order.as<uint32_t>(), hb); JF_LAUNCHED();
           win_scan_kernel<<<1, 1024, 0, st>>>(wd, T0.stats); JF_LAUNCHED();
-          win_event(e, st);
+          CUDA_OK(e, win_event(e, st));
           win_scatter_kernel<false><<<std::min<uint32_t>(stiles, e->n_sm * 2), WIN_ST_NTH, scatter_smem, st>>>(pd, wd, ps.order.as<uint32_t>(), hb);
           JF_LAUNCHED();
-          win_event(e, st);
+          CUDA_OK(e, win_event(e, st));
           if(e->kw == 1) {
             cudaFuncSetAttribute(win_insert2_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WIN2_SMEM);
             win_insert2_kernel<1><<<e->n_sm, WIN2_NTH, WIN2_SMEM, st>>>(T0, pd, wd, e->tab.inv_lut.as<uint64_t>(), e->nbytes); JF_LAUNCHED();
@@ -770,7 +810,7 @@ int part_drain(jfgpu_engine* e, cudaStream_t st) {
             JF_LAUNCHED();
           }
           settle();
-          win_event(e, st);
+          CUDA_OK(e, win_event(e, st));
         } else {
           if(zero) {
             win_zero_kernel<<<e->n_sm * 4, 256, 0, st>>>(e->tab.slots.as<uint32_t>(), wd.lazy_win, nullptr, (uint64_t)r0 << wpr_lg, G << wpr_lg);
@@ -821,7 +861,10 @@ int part_drain(jfgpu_engine* e, cudaStream_t st) {
   { float ms = 0; if(cudaEventElapsedTime(&ms, e->ev_d0, e->ev_d1) == cudaSuccess) e->drain_ms += ms; else cudaGetLastError(); }
   resolve_win_events(e, st);
   ps.pending = false;
-  if(rebuilt) { cudaStreamSynchronize(st); old_inv.free(); part_configure(e); if(!e->part.P) part_release(e); }
+  if(rebuilt) {                  // (old_inv goes when the drain returns; the stream is idle)
+    part_configure(e);
+    if(!ps.P) ps = PartState();  // a table no longer filled region by region gives its record pool back
+  }
   ps.bound_chunks = ps.P;
   if(rc) return rc;
   CUDA_OK(e, cudaGetLastError());
@@ -943,7 +986,11 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
     const int sms = shard_send && e->n_sm > 32 ? e->n_sm - (int)SHARD_RESERVED_SMS : e->n_sm;
     const int grid = (int)std::min<uint64_t>(n_tiles, (uint64_t)sms * per_sm);
     if(query) { kern<<<grid, nth, smem, stream>>>(a, pd); return JFGPU_OK; }     // (the counting statistics leave a query out)
-    if(e->kev_used + 2 > e->kev.size()) { cudaEvent_t a0, a1; cudaEventCreate(&a0); cudaEventCreate(&a1); e->kev.push_back(a0); e->kev.push_back(a1); }
+    if(e->kev_used == e->kev.size()) e->kev.resize(e->kev_used + 2);
+    if(!e->kev[e->kev_used]) {
+      c = make_all(need(e->kev[e->kev_used], cudaEventDefault), need(e->kev[e->kev_used + 1], cudaEventDefault));
+      if(c != cudaSuccess) return fail(e, JFGPU_ERR_CUDA, std::string("cudaEventCreate: ") + cudaGetErrorString(c));
+    }
     cudaEventRecord(e->kev[e->kev_used], stream);
     kern<<<grid, nth, smem, stream>>>(a, pd);
     cudaEventRecord(e->kev[e->kev_used + 1], stream);
@@ -1079,7 +1126,6 @@ int insert_keys_into(jfgpu_engine* e, Table& t, const uint64_t* keys, const uint
 struct SegScratch {
   DevBuf keys, counts, sort_lo, n_out;
   uint64_t cap = 0;
-  void free_all() { keys.free(); counts.free(); sort_lo.free(); n_out.free(); cap = 0; }
 };
 
 int seg_alloc(jfgpu_engine* e, SegScratch& s, uint64_t cap) {
@@ -1141,11 +1187,9 @@ struct ForceCount {
 
 // Turn to the other failure list (allocated on first use), so that the failures of a re-insertion are kept apart.
 int flip_fail_list(jfgpu_engine* e) {
-  e->fail_cur ^= 1;
-  if(!e->fail_keys[e->fail_cur].p) {
-    CUDA_OK(e, e->fail_keys[e->fail_cur].alloc(e->fail_cap * 8 * e->kw));
-    CUDA_OK(e, e->fail_counts[e->fail_cur].alloc(e->fail_cap * 8));
-  }
+  const int next = e->fail_cur ^ 1;
+  if(!e->fail_keys[next].p) CUDA_OK(e, make_all(need(e->fail_keys[next], e->fail_cap * 8 * e->kw), need(e->fail_counts[next], e->fail_cap * 8)));
+  e->fail_cur = next;
   return JFGPU_OK;
 }
 
@@ -1155,9 +1199,9 @@ int rebuild_table(jfgpu_engine* e, unsigned nl, const jfb::gf2_matrix& M, int ol
   const ForceCount force_count(e);
   Table nt;
   int rc = table_setup(e, nt, nl, M, e->tab.max_reprobe);
-  if(rc) { nt.release(); return rc == JFGPU_ERR_NOMEM ? fail(e, JFGPU_ERR_FULL, "Hash full (" + e->err + ")") : rc; }
+  if(rc) return rc == JFGPU_ERR_NOMEM ? fail(e, JFGPU_ERR_FULL, "Hash full (" + e->err + ")") : rc;
   rc = table_zero(e, nt, false);
-  if(rc) { nt.release(); return rc; }
+  if(rc) return rc;
   // distinct / reprobes statistics restart for the new table; STAT_INSERTED counts k-mer
   // occurrences and must not change
   unsigned long long inserted_before = 0;
@@ -1165,29 +1209,29 @@ int rebuild_table(jfgpu_engine* e, unsigned nl, const jfb::gf2_matrix& M, int ol
   CUDA_OK(e, cudaStreamSynchronize(e->cs));
   CUDA_OK(e, cudaMemsetAsync(e->stats.as<unsigned long long>() + STAT_DISTINCT, 0, 8, e->cs));
   CUDA_OK(e, cudaMemsetAsync(e->stats.as<unsigned long long>() + STAT_REPROBES, 0, 8, e->cs));
-  SegScratch s;
-  const uint64_t seg = pick_segment(e->tab);
-  rc = seg_alloc(e, s, seg + e->tab.margin + 8);
-  for(uint64_t lo = 0; lo < e->tab.local_size && !rc; lo += seg) {
-    uint64_t n = 0;
-    rc = collect_segment(e, e->tab, s, lo, std::min(lo + seg, e->tab.local_size), 0, ~0ull, &n);
-    if(!rc) rc = insert_keys_into(e, nt, s.keys.as<uint64_t>(), s.counts.as<uint64_t>(), n, e->cs);
+  {
+    SegScratch s;                // (goes at the end of this block, before the failed keys are inserted)
+    const uint64_t seg = pick_segment(e->tab);
+    rc = seg_alloc(e, s, seg + e->tab.margin + 8);
+    for(uint64_t lo = 0; lo < e->tab.local_size && !rc; lo += seg) {
+      uint64_t n = 0;
+      rc = collect_segment(e, e->tab, s, lo, std::min(lo + seg, e->tab.local_size), 0, ~0ull, &n);
+      if(!rc) rc = insert_keys_into(e, nt, s.keys.as<uint64_t>(), s.counts.as<uint64_t>(), n, e->cs);
+    }
+    cudaStreamSynchronize(e->cs);
   }
-  cudaStreamSynchronize(e->cs);
-  s.free_all();
-  if(rc) { nt.release(); return rc; }
+  if(rc) return rc;
   // the moved entries are not new k-mer occurrences; the failed ones (below) are
   CUDA_OK(e, cudaMemcpyAsync(e->stats.as<unsigned long long>() + STAT_INSERTED, &inserted_before, 8, cudaMemcpyHostToDevice, e->cs));
   CUDA_OK(e, cudaStreamSynchronize(e->cs));
   if(n_failed) {
     rc = insert_keys_into(e, nt, e->fail_keys[old_fail].as<uint64_t>(), e->fail_counts[old_fail].as<uint64_t>(), n_failed, e->cs);
     cudaStreamSynchronize(e->cs);
-    if(rc) { nt.release(); return rc; }
+    if(rc) return rc;
   }
   // (each table owns its counter-carry side table: the old one dies with the old slots)
-  e->tab.release();
-  e->tab = nt;
-  if(!e->part.pending) { part_configure(e); if(!e->part.P) part_release(e); }
+  e->tab = std::move(nt);
+  if(!e->part.pending) { part_configure(e); if(!e->part.P) e->part = PartState(); }
   return JFGPU_OK;
 }
 
@@ -1378,18 +1422,18 @@ int jfgpu_create(const jfgpu_params* params, jfgpu_handle* out) {
   if((c = cudaGetDeviceProperties(&prop, e->device)) != cudaSuccess) { e->err = cudaGetErrorString(c); return bail(JFGPU_ERR_CUDA); }
   if(prop.major != 9 || prop.minor != 0) { e->err = "this engine is built for sm_90a (Hopper) only"; return bail(JFGPU_ERR_CUDA); }
   e->n_sm = prop.multiProcessorCount;
-  if(cudaStreamCreateWithFlags(&e->cs, cudaStreamNonBlocking) != cudaSuccess ||
-     cudaStreamCreateWithFlags(&e->hs, cudaStreamNonBlocking) != cudaSuccess) { e->err = "stream creation failed"; return bail(JFGPU_ERR_CUDA); }
-  cudaEventCreate(&e->ev_t0); cudaEventCreate(&e->ev_t1);
-  cudaHostAlloc((void**)&e->h_watch, 16, cudaHostAllocDefault);
-  for(int i = 0; i < 2; ++i) cudaEventCreateWithFlags(&e->ev_watch[i], cudaEventDisableTiming);
-  for(int i = 0; i < 2; ++i) { cudaEventCreateWithFlags(&e->ev_copied[i], cudaEventDisableTiming); cudaEventCreateWithFlags(&e->ev_done[i], cudaEventDisableTiming); }
+  if(e->cs.create() != cudaSuccess || e->hs.create() != cudaSuccess) { e->err = "stream creation failed"; return bail(JFGPU_ERR_CUDA); }
+  const unsigned untimed = cudaEventDisableTiming;
+  if(make_all(need(e->ev_t0, cudaEventDefault), need(e->ev_t1, cudaEventDefault), need(e->ev_watch[0], untimed), need(e->ev_watch[1], untimed),
+              need(e->ev_copied[0], untimed), need(e->ev_copied[1], untimed), need(e->ev_done[0], untimed), need(e->ev_done[1], untimed)) != cudaSuccess) {
+    e->err = "event creation failed";
+    return bail(JFGPU_ERR_CUDA);
+  }
 
   if(params->bloom_counter) {
     // `jellyfish bc`: no hash table at all; the two hash matrices are the FIRST draws of the random stream (bc_main.cc:103-106)
-    bool ok0 = e->stats.alloc(STAT_N * 8) == cudaSuccess && e->carry[0].alloc(sizeof(Carry)) == cudaSuccess && e->carry[1].alloc(sizeof(Carry)) == cudaSuccess &&
-               cudaHostAlloc((void**)&e->h_stats, STAT_N * 8, cudaHostAllocDefault) == cudaSuccess;
-    if(!ok0) { cudaGetLastError(); e->err = "device allocation failed"; return bail(JFGPU_ERR_NOMEM); }
+    if(make_all(need(e->stats, STAT_N * 8), need(e->carry[0], sizeof(Carry)), need(e->carry[1], sizeof(Carry)), need(e->h_stats, STAT_N * 8),
+                need(e->h_watch, 16)) != cudaSuccess) { e->err = "device allocation failed"; return bail(JFGPU_ERR_NOMEM); }
     cudaMemsetAsync(e->stats.p, 0, STAT_N * 8, e->cs);
     memset(e->h_stats, 0, STAT_N * 8);
     e->batch_bytes = params->max_batch_bytes ? (size_t)((params->max_batch_bytes + 15) & ~(uint64_t)15) : ((size_t)64 << 20);
@@ -1418,11 +1462,9 @@ int jfgpu_create(const jfgpu_params* params, jfgpu_handle* out) {
   // at most a group).
   e->fail_group = e->batch_bytes;
   e->fail_cap = 2 * e->fail_group + std::min<uint64_t>(WIN_DEF_CAP, e->fail_group);
-  bool ok = e->stats.alloc(STAT_N * 8) == cudaSuccess && e->carry[0].alloc(sizeof(Carry)) == cudaSuccess &&
-            e->carry[1].alloc(sizeof(Carry)) == cudaSuccess &&
-            e->fail_keys[0].alloc(e->fail_cap * 8 * e->kw) == cudaSuccess && e->fail_counts[0].alloc(e->fail_cap * 8) == cudaSuccess &&
-            cudaHostAlloc((void**)&e->h_stats, STAT_N * 8, cudaHostAllocDefault) == cudaSuccess;
-  if(!ok) { cudaGetLastError(); e->err = "device allocation failed"; return bail(JFGPU_ERR_NOMEM); }
+  if(make_all(need(e->stats, STAT_N * 8), need(e->carry[0], sizeof(Carry)), need(e->carry[1], sizeof(Carry)),
+              need(e->fail_keys[0], e->fail_cap * 8 * e->kw), need(e->fail_counts[0], e->fail_cap * 8), need(e->h_stats, STAT_N * 8),
+              need(e->h_watch, 16)) != cudaSuccess) { e->err = "device allocation failed"; return bail(JFGPU_ERR_NOMEM); }
   cudaMemsetAsync(e->stats.p, 0, STAT_N * 8, e->cs);
   memset(e->h_stats, 0, STAT_N * 8);
   int rc = table_setup(e, e->tab, lsize, M, params->max_reprobe);
@@ -1444,40 +1486,7 @@ void jfgpu_destroy(jfgpu_handle e) {
   cudaSetDevice(e->device);
   if(e->cs) cudaStreamSynchronize(e->cs);
   if(e->hs) cudaStreamSynchronize(e->hs);
-  e->tab.release();
-  part_release(e);
-  e->bloom.release();
-  e->sh.pool_next[0].free(); e->sh.pool_next[1].free(); e->sh.cta_chunk.free(); e->sh.cta_fill.free();
-  if(e->sh.h_counts) cudaFreeHost(e->sh.h_counts);
-  e->stats.free();
-  for(int i = 0; i < 2; ++i) {
-    e->carry[i].free(); e->fail_keys[i].free(); e->fail_counts[i].free(); e->stage[i].free();
-    if(e->ev_copied[i]) cudaEventDestroy(e->ev_copied[i]);
-    if(e->ev_done[i]) cudaEventDestroy(e->ev_done[i]);
-  }
-  e->nlA.free(); e->nlB.free(); e->cntA.free(); e->cntB.free(); e->tstate.free();
-  for(int i = 0; i < 2; ++i) {
-    jfgpu_engine::QueryBufs& q = e->qb[i];
-    q.keys.free(); q.vals.free(); q.cnt.free(); q.off.free(); q.out.free();
-    if(q.h_off) cudaFreeHost(q.h_off);
-    if(q.h_cnt) cudaFreeHost(q.h_cnt);
-    if(q.ev_front) cudaEventDestroy(q.ev_front);
-    if(q.ev_fmt) cudaEventDestroy(q.ev_fmt);
-    if(e->q_host[i]) cudaFreeHost(e->q_host[i]);
-    if(e->ev_qcopy[i]) cudaEventDestroy(e->ev_qcopy[i]);
-  }
-  if(e->h_stats) cudaFreeHost(e->h_stats);
-  if(e->h_watch) cudaFreeHost(e->h_watch);
-  for(int i = 0; i < 2; ++i) if(e->ev_watch[i]) cudaEventDestroy(e->ev_watch[i]);
-  if(e->ev_t0) cudaEventDestroy(e->ev_t0);
-  if(e->ev_t1) cudaEventDestroy(e->ev_t1);
-  if(e->ev_d0) cudaEventDestroy(e->ev_d0);
-  if(e->ev_d1) cudaEventDestroy(e->ev_d1);
-  for(cudaEvent_t ev : e->kev) cudaEventDestroy(ev);
-  for(cudaEvent_t ev : e->wev) cudaEventDestroy(ev);
-  if(e->cs) cudaStreamDestroy(e->cs);
-  if(e->hs) cudaStreamDestroy(e->hs);
-  delete e;
+  delete e;                      // (every buffer, event and stream is released by its owner, the streams last)
 }
 
 static int begin_feed(jfgpu_engine* e, uint32_t flags, int first_byte, cudaStream_t st) {
@@ -1691,10 +1700,9 @@ int jfgpu_shard_setup(jfgpu_handle e, const jfgpu_shard_buffers* b) {
   sh.P = P; sh.sbits = sbits; sh.own_regions = P / G; sh.owner_shift = ceil_log2(P / G); sh.split_lg = sbits - e->part.region_bits;
   sh.arena_chunks = b->send_arena_chunks; sh.seg_chunks = b->recv_seg_chunks;
   sh.send_pool = (uint8_t*)b->send_pool; sh.send_dir = (uint2*)b->send_dir; sh.recv_pool = (uint8_t*)b->recv_pool; sh.recv_dir = (uint2*)b->recv_dir;
-  bool ok = sh.pool_next[0].alloc(((size_t)G + 2) * 4) == cudaSuccess && sh.pool_next[1].alloc(((size_t)G + 2) * 4) == cudaSuccess &&
-            sh.cta_chunk.alloc((size_t)e->n_sm * RING_P * 4) == cudaSuccess && sh.cta_fill.alloc((size_t)e->n_sm * RING_P * 4) == cudaSuccess &&
-            (sh.h_counts || cudaHostAlloc((void**)&sh.h_counts, 16 * sizeof(unsigned int), cudaHostAllocDefault) == cudaSuccess);
-  if(!ok) { cudaGetLastError(); return fail(e, JFGPU_ERR_NOMEM, "device allocation failed"); }
+  if(make_all(need(sh.pool_next[0], ((size_t)G + 2) * 4), need(sh.pool_next[1], ((size_t)G + 2) * 4), need(sh.cta_chunk, (size_t)e->n_sm * RING_P * 4),
+              need(sh.cta_fill, (size_t)e->n_sm * RING_P * 4), need(sh.h_counts, 16 * sizeof(unsigned int))) != cudaSuccess)
+    return fail(e, JFGPU_ERR_NOMEM, "device allocation failed");
   for(int i = 0; i < 2; ++i) CUDA_OK(e, cudaMemsetAsync(sh.pool_next[i].p, 0, sh.pool_next[i].bytes, e->cs));
   CUDA_OK(e, cudaMemsetAsync(sh.cta_chunk.p, 0xFF, sh.cta_chunk.bytes, e->cs));
   CUDA_OK(e, cudaMemsetAsync(sh.cta_fill.p, 0, sh.cta_fill.bytes, e->cs));
@@ -1948,15 +1956,14 @@ int jfgpu_dump(jfgpu_handle e, uint64_t lower, uint64_t upper, uint32_t ocl, jfg
   const uint64_t cap = seg + t.margin + 8;                    // records of a segment at most
   const uint32_t max_tiles = (uint32_t)((seg + DUMP_TP - 1) / DUMP_TP);
   DevBuf tile_cnt[2], out[2];
-  uint8_t* hbuf[2] = { nullptr, nullptr };
-  uint32_t* h_total = nullptr;
-  cudaEvent_t ev_emit[2] = { nullptr, nullptr }, ev_copy[2] = { nullptr, nullptr };
-  bool ok = cudaHostAlloc((void**)&h_total, 2 * sizeof(uint32_t), cudaHostAllocDefault) == cudaSuccess;
-  for(int i = 0; i < 2 && ok; ++i)
-    ok = tile_cnt[i].alloc(((size_t)max_tiles + 1) * 4) == cudaSuccess && out[i].alloc(cap * rec + 16) == cudaSuccess &&
-         cudaHostAlloc((void**)&hbuf[i], cap * rec + 16, cudaHostAllocDefault) == cudaSuccess &&
-         cudaEventCreateWithFlags(&ev_emit[i], cudaEventDisableTiming) == cudaSuccess && cudaEventCreateWithFlags(&ev_copy[i], cudaEventDisableTiming) == cudaSuccess;
-  if(!ok) { cudaGetLastError(); rc = fail(e, JFGPU_ERR_NOMEM, "allocation of the dump buffers failed"); }
+  HostBuf<uint8_t> hbuf[2];
+  HostBuf<uint32_t> h_total;
+  Event ev_emit[2], ev_copy[2];
+  const unsigned untimed = cudaEventDisableTiming;
+  if(make_all(need(h_total, 2 * sizeof(uint32_t)),
+              need(tile_cnt[0], ((size_t)max_tiles + 1) * 4), need(out[0], cap * rec + 16), need(hbuf[0], cap * rec + 16), need(ev_emit[0], untimed), need(ev_copy[0], untimed),
+              need(tile_cnt[1], ((size_t)max_tiles + 1) * 4), need(out[1], cap * rec + 16), need(hbuf[1], cap * rec + 16), need(ev_emit[1], untimed), need(ev_copy[1], untimed))
+     != cudaSuccess) rc = fail(e, JFGPU_ERR_NOMEM, "allocation of the dump buffers failed");
   const size_t smem = (size_t)e->nbytes * 256 * 8 + ((size_t)DUMP_TP + 1) * 4 + (size_t)DUMP_MAXC * 2 + (size_t)DUMP_NTH * rec;
   uint64_t total = 0;
   const uint64_t n_seg = (t.local_size + seg - 1) / seg;
@@ -2005,14 +2012,7 @@ int jfgpu_dump(jfgpu_handle e, uint64_t lower, uint64_t upper, uint32_t ocl, jfg
     if(n_in_buf[b] && sink(ctx, hbuf[b], n_in_buf[b] * rec) != 0) { rc = fail(e, JFGPU_ERR_SINK, "dump sink failed"); break; }
     total += n_in_buf[b];
   }
-  cudaStreamSynchronize(e->cs); cudaStreamSynchronize(e->hs);
-  for(int i = 0; i < 2; ++i) {
-    tile_cnt[i].free(); out[i].free();
-    if(hbuf[i]) cudaFreeHost(hbuf[i]);
-    if(ev_emit[i]) cudaEventDestroy(ev_emit[i]);
-    if(ev_copy[i]) cudaEventDestroy(ev_copy[i]);
-  }
-  if(h_total) cudaFreeHost(h_total);
+  cudaStreamSynchronize(e->cs); cudaStreamSynchronize(e->hs);      // (before the buffers go)
   if(n_records) *n_records = total;
   return rc;
 }
@@ -2042,7 +2042,6 @@ int jfgpu_lookup(jfgpu_handle e, const uint64_t* keys, size_t n, uint64_t* vals)
     if(c == cudaSuccess) c = cudaStreamSynchronize(e->cs);
     if(c != cudaSuccess) rc = fail(e, JFGPU_ERR_CUDA, std::string("lookup: ") + cudaGetErrorString(c));
   }
-  dk.free(); dv.free();
   return rc;
 }
 
@@ -2066,14 +2065,10 @@ int jfgpu_load_records(jfgpu_handle e, const void* records, size_t nbytes, uint3
   const uint64_t n_rec = nbytes / rec;
   // a slice is at most one group of the failure list (regrow re-inserts what found no slot)
   const uint64_t slice = std::min<uint64_t>(std::min<uint64_t>(((uint64_t)64 << 20) / rec, e->fail_group), n_rec);
-  uint8_t* h[2] = { nullptr, nullptr };
+  HostBuf<uint8_t> h[2];
   DevBuf raw, keys, counts;
-  bool ok = raw.alloc(slice * rec + 16) == cudaSuccess && keys.alloc(slice * 8 * e->kw) == cudaSuccess && counts.alloc(slice * 8) == cudaSuccess;
-  for(int i = 0; i < 2 && ok; ++i) ok = cudaHostAlloc((void**)&h[i], slice * rec, cudaHostAllocDefault) == cudaSuccess;
-  if(!ok) {
-    cudaGetLastError();
+  if(make_all(need(raw, slice * rec + 16), need(keys, slice * 8 * e->kw), need(counts, slice * 8), need(h[0], slice * rec), need(h[1], slice * rec)) != cudaSuccess)
     rc = fail(e, JFGPU_ERR_NOMEM, "allocation of the load staging buffers failed");
-  }
   ForceCount force_count(e);                    // the records' counts are added, whatever the counter is doing
   const uint8_t* src = (const uint8_t*)records;
   if(!rc) memcpy(h[0], src, slice * rec);
@@ -2093,9 +2088,7 @@ int jfgpu_load_records(jfgpu_handle e, const void* records, size_t nbytes, uint3
     if(first + m < n_rec) memcpy(h[b ^ 1], src + (first + m) * rec, std::min(slice, n_rec - first - m) * rec);
     rc = check_after_batches(e);                // (synchronises; a table that is full is doubled, counts and all)
   }
-  cudaStreamSynchronize(e->cs);
-  raw.free(); keys.free(); counts.free();
-  for(int i = 0; i < 2; ++i) if(h[i]) cudaFreeHost(h[i]);
+  cudaStreamSynchronize(e->cs);                 // (before the staging buffers go)
   // (a full carry side table is not a lack of memory: a larger table would not get a larger one below 2^26 slots)
   if(rc == JFGPU_ERR_FULL && !e->h_stats[STAT_OVF_FULL]) rc = fail(e, JFGPU_ERR_NOMEM, "the database does not fit in device memory (" + e->err + ")");
   return rc;
@@ -2114,19 +2107,15 @@ static int query_impl(jfgpu_engine* e, const char* bytes, size_t n, uint32_t fla
   const size_t PIECE = (size_t)64 << 20;        // bytes handed to the sink at most (whole windows: one window's lines < 1.4 MB)
   if(e->q_tiles_cap < max_tiles) {
     CUDA_OK(e, cudaStreamSynchronize(e->cs));
+    e->q_tiles_cap = 0;
+    const unsigned untimed = cudaEventDisableTiming;
     for(int i = 0; i < 2; ++i) {
       jfgpu_engine::QueryBufs& q = e->qb[i];
-      if(q.h_off) { cudaFreeHost(q.h_off); q.h_off = nullptr; }
-      if(q.h_cnt) { cudaFreeHost(q.h_cnt); q.h_cnt = nullptr; }
-      bool ok = q.keys.alloc(max_tiles * TILE * 8 * e->kw) == cudaSuccess && q.vals.alloc(max_tiles * TILE * 8) == cudaSuccess &&
-                q.cnt.alloc(max_tiles * 4) == cudaSuccess && q.off.alloc((max_tiles + 1) * 8) == cudaSuccess &&
-                cudaHostAlloc((void**)&q.h_off, (max_tiles + 1) * 8, cudaHostAllocDefault) == cudaSuccess &&
-                cudaHostAlloc((void**)&q.h_cnt, max_tiles * 4, cudaHostAllocDefault) == cudaSuccess;
-      if(ok && !q.ev_front) ok = cudaEventCreateWithFlags(&q.ev_front, cudaEventDisableTiming) == cudaSuccess &&
-                                 cudaEventCreateWithFlags(&q.ev_fmt, cudaEventDisableTiming) == cudaSuccess;
-      if(ok && !e->q_host[i]) ok = cudaHostAlloc((void**)&e->q_host[i], PIECE, cudaHostAllocDefault) == cudaSuccess &&
-                                   cudaEventCreateWithFlags(&e->ev_qcopy[i], cudaEventDisableTiming) == cudaSuccess;
-      if(!ok) { cudaGetLastError(); return fail(e, JFGPU_ERR_NOMEM, "allocation of the query buffers failed"); }
+      cudaError_t c = make_all(need(q.keys, max_tiles * TILE * 8 * e->kw), need(q.vals, max_tiles * TILE * 8), need(q.cnt, max_tiles * 4),
+                               need(q.off, (max_tiles + 1) * 8), need(q.h_off, (max_tiles + 1) * 8), need(q.h_cnt, max_tiles * 4));
+      if(c == cudaSuccess && !q.ev_front) c = make_all(need(q.ev_front, untimed), need(q.ev_fmt, untimed));
+      if(c == cudaSuccess && !e->q_host[i]) c = make_all(need(e->q_host[i], PIECE), need(e->ev_qcopy[i], untimed));
+      if(c != cudaSuccess) return fail(e, JFGPU_ERR_NOMEM, "allocation of the query buffers failed");
     }
     e->q_tiles_cap = max_tiles;
   }
@@ -2254,7 +2243,6 @@ int jfgpu_histogram(jfgpu_handle e, uint64_t* hist, uint32_t n_bins) {
   JF_LAUNCHED();
   cudaError_t c = cudaMemcpyAsync(hist, dh.p, (size_t)n_bins * 8, cudaMemcpyDeviceToHost, e->cs);
   if(c == cudaSuccess) c = cudaStreamSynchronize(e->cs);
-  dh.free();
   if(c != cudaSuccess) return fail(e, JFGPU_ERR_CUDA, std::string("histogram: ") + cudaGetErrorString(c));
   return JFGPU_OK;
 }
@@ -2287,17 +2275,16 @@ int jfgpu_bloom_load(jfgpu_handle e, uint64_t m, uint32_t nb_hashes, const uint6
   b.m = m; b.k = nb_hashes;
   b.inv = m == 1 ? ~(uint64_t)0 : (uint64_t)(((unsigned __int128)1 << 64) / m);
   b.n_words = (m + 31) / 32;
-  DevBuf raw;
-  const size_t nb = m / 5 + (m % 5 != 0);
-  if(b.bits.alloc((size_t)b.n_words * 4 + 16) != cudaSuccess || raw.alloc(nb + 16) != cudaSuccess) {
-    cudaGetLastError(); b.bits.free(); raw.free();
-    return fail(e, JFGPU_ERR_NOMEM, "Failed to allocate the Bloom counter in device memory");
+  {
+    DevBuf raw;                  // (goes at the end of this block, before the hash tables are uploaded)
+    const size_t nb = m / 5 + (m % 5 != 0);
+    if(make_all(need(b.bits, (size_t)b.n_words * 4 + 16), need(raw, nb + 16)) != cudaSuccess)
+      return fail(e, JFGPU_ERR_NOMEM, "Failed to allocate the Bloom counter in device memory");
+    CUDA_OK(e, cudaMemcpyAsync(raw.p, bytes, nb, cudaMemcpyHostToDevice, e->cs));
+    const int grid = (int)std::min<uint64_t>((b.n_words + 255) / 256, (uint64_t)e->n_sm * 16);
+    bloom_unpack_kernel<<<grid, 256, 0, e->cs>>>(raw.as<uint8_t>(), m, b.n_words, b.bits.as<uint32_t>()); JF_LAUNCHED();
+    CUDA_OK(e, cudaStreamSynchronize(e->cs));
   }
-  CUDA_OK(e, cudaMemcpyAsync(raw.p, bytes, nb, cudaMemcpyHostToDevice, e->cs));
-  const int grid = (int)std::min<uint64_t>((b.n_words + 255) / 256, (uint64_t)e->n_sm * 16);
-  bloom_unpack_kernel<<<grid, 256, 0, e->cs>>>(raw.as<uint8_t>(), m, b.n_words, b.bits.as<uint32_t>()); JF_LAUNCHED();
-  CUDA_OK(e, cudaStreamSynchronize(e->cs));
-  raw.free();
   b.M1 = jfb::gf2_matrix(64, 2 * e->k, c1); b.M2 = jfb::gf2_matrix(64, 2 * e->k, c2);
   b.mode = BLOOM_CHECK;
   return bloom_upload_matrices(e);
@@ -2312,11 +2299,8 @@ int jfgpu_bloom_dump(jfgpu_handle e, jfgpu_sink_fn sink, void* ctx) {
   if(rc) return rc;
   const uint64_t nb = b.m / 5 + (b.m % 5 != 0);
   const uint64_t piece = (uint64_t)64 << 20;
-  DevBuf out; uint8_t* hbuf = nullptr;
-  if(out.alloc(piece) != cudaSuccess || cudaHostAlloc((void**)&hbuf, piece, cudaHostAllocDefault) != cudaSuccess) {
-    cudaGetLastError(); out.free();
-    return fail(e, JFGPU_ERR_NOMEM, "allocation of the Bloom counter staging buffers failed");
-  }
+  DevBuf out; HostBuf<uint8_t> hbuf;
+  if(make_all(need(out, piece), need(hbuf, piece)) != cudaSuccess) return fail(e, JFGPU_ERR_NOMEM, "allocation of the Bloom counter staging buffers failed");
   for(uint64_t off = 0; off < nb && !rc; off += piece) {
     const uint64_t len = std::min(piece, nb - off);
     const int grid = (int)std::min<uint64_t>((len + 255) / 256, (uint64_t)e->n_sm * 16);
@@ -2327,7 +2311,6 @@ int jfgpu_bloom_dump(jfgpu_handle e, jfgpu_sink_fn sink, void* ctx) {
     if(c != cudaSuccess) { rc = fail(e, JFGPU_ERR_CUDA, std::string("bloom dump: ") + cudaGetErrorString(c)); break; }
     if(sink(ctx, hbuf, len) != 0) rc = fail(e, JFGPU_ERR_SINK, "dump sink failed");
   }
-  cudaFreeHost(hbuf); out.free();
   return rc;
 }
 

@@ -11,7 +11,10 @@ are drawn from fixed seeds.
 The scenarios cover the region-by-region paths: the window form of K2 at k2_mode 0, 3 and 4 and a second drain into a
 table in memory, the L2 forms at k2_mode 1 and 2, a doubling in the middle of a write-only drain and in the L2 form, a
 full spill list before the first drain, PRIME / UPDATE, routed keys staged by insert_keys, the record exchange
-(shard_extract / pack / unpack), text fed from host and from device memory, query, and k = 63 in 128-bit slots.
+(shard_extract / pack / unpack), text fed from host and from device memory, query, and k = 63 in 128-bit slots.  They
+also cover the calls that hold buffers of their own: dump, lookup and histogram at k = 21 and k = 100 (the wide
+kernels), a database loaded with a doubling in the middle and then queried, count --bf-size, and a Bloom counter built,
+dumped and loaded back in front of a table.
 """
 import json
 import os
@@ -31,9 +34,9 @@ def fasta(n, seed, period=0):
     return b">r\n" + b"\n".join(seq[i:i + 70] for i in range(0, n, 70)) + b"\n"
 
 
-def scenarios():
+def scenarios(tmp):
     import torch
-    from jellyfish_b200 import HashCounter
+    from jellyfish_b200 import BloomCounter, HashCounter, load_database
     from jellyfish_b200.distributed import CHUNK
 
     def win(**kw):            # k=17, 2^23 32-bit slots, 256 regions, 4-byte records: the window form under part_min_mb=1
@@ -139,10 +142,57 @@ def scenarios():
             assert hc.info()["slot_bits"] == 128
             hc.add_text(fasta(1_000_000, 513)); hc.done()
 
+    def dump_lookup_histogram(k):
+        def run():
+            with HashCounter(2_000_000, 7, k=k, canonical=True, max_batch_bytes=1 << 20) as hc:
+                hc.add_text(fasta(1_000_000, 514)); hc.done()
+                hc.dump_records(sink="discard")
+                hc.get_many(list(range(1000)))
+                hc.histogram()
+        return run
+
+    def database():
+        """a k=21 database of about 900k distinct k-mers"""
+        path = os.path.join(tmp, "db.jf")
+        with HashCounter(4_000_000, 7, k=21, canonical=True, max_batch_bytes=1 << 20) as hc:
+            hc.add_text(fasta(1_000_000, 515)); hc.done()
+            hc.dump(path)
+        return path
+
+    def load_with_doubling():
+        hc = load_database(database(), size=1 << 17, max_batch_bytes=1 << 20)      # the table doubles while it loads
+        try:
+            assert hc.info()["size"] > 1 << 17
+        finally:
+            hc.close()
+
+    def query_database():
+        hc = load_database(database(), max_batch_bytes=1 << 20)
+        try:
+            hc.query_text(fasta(300_000, 516))
+        finally:
+            hc.close()
+
+    def bloom_filter():
+        with HashCounter(2_000_000, 7, k=21, canonical=True, bf_size=2_000_000, max_batch_bytes=1 << 20) as hc:
+            hc.add_text(fasta(1_000_000, 517)); hc.done()
+
+    def bloom_counter():
+        path = os.path.join(tmp, "bc.bin")
+        with BloomCounter(2_000_000, k=21, canonical=True, max_batch_bytes=1 << 20) as bc:
+            bc.add_text(fasta(1_000_000, 518))
+            bc.dump(path)
+        with HashCounter(2_000_000, 7, k=21, canonical=True, max_batch_bytes=1 << 20) as hc:
+            hc.load_bloom_counter(path)
+            hc.add_text(fasta(1_000_000, 518)); hc.done()
+
     return [("window_k2_mode_%d" % m, window(m)) for m in (0, 3, 4)] + [("l2_k2_mode_%d" % m, l2(m)) for m in (1, 2)] + [
         ("regrow_in_write_only_drain", lazy_regrow), ("full_spill_list", spill_list), ("regrow_l2_form", l2_regrow),
         ("prime_update", prime_update), ("device_text", device_text), ("route_insert_keys", route_insert_keys),
-        ("record_exchange", record_exchange), ("query", query), ("k63_128bit_slots", k63_wide_slots)]
+        ("record_exchange", record_exchange), ("query", query), ("k63_128bit_slots", k63_wide_slots),
+        ("dump_lookup_histogram_k21", dump_lookup_histogram(21)), ("dump_lookup_histogram_k100", dump_lookup_histogram(100)),
+        ("load_database_doubling", load_with_doubling), ("query_loaded_database", query_database),
+        ("count_bf_size", bloom_filter), ("bloom_counter_dump_load", bloom_counter)]
 
 
 def kernels(trace_path):
@@ -162,7 +212,7 @@ def main():
     from torch.profiler import ProfilerActivity, profile
     torch.zeros(1, device="cuda")
     with tempfile.TemporaryDirectory() as d:
-        for name, run in scenarios():
+        for name, run in scenarios(d):
             torch.cuda.synchronize()
             n0 = lib.jfgpu_kernel_launches()
             with profile(activities=[ProfilerActivity.CUDA]) as prof:
