@@ -274,7 +274,33 @@ int  jfgpu_histogram(jfgpu_handle h, uint64_t* hist, uint32_t n_bins);
 int  jfgpu_bloom_info_get(jfgpu_handle h, jfgpu_bloom_info* info);
 int  jfgpu_bloom_load(jfgpu_handle h, uint64_t m, uint32_t nb_hashes, const uint64_t* matrix1_cols, const uint64_t* matrix2_cols,
                       const void* bytes, size_t nbytes);
-int  jfgpu_bloom_dump(jfgpu_handle h, jfgpu_sink_fn sink, void* ctx);
+int  jfgpu_bloom_dump(jfgpu_handle h, jfgpu_sink_fn sink, void* ctx);   /* = jfgpu_bloom_dump_range over the whole body */
+
+/* -- Bloom structures on the sharded path (no reference analogue: `jellyfish bc` and `count --bf-size/--bc` are one process)
+ *    count --bc: every shard loads the whole counter (jfgpu_bloom_load) and jfgpu_extract_route drops a k-mer that fails it
+ *    before bucketing it (filter_bc is a read-only test, count_main.cc:110-120).  The loaded form takes 1 bit per position:
+ *    m / 8 bytes per shard, e.g. `bc -s 5G` at the default -f 0.001 (m = 14 bits per k-mer) 8.75 GB on every rank.
+ *    count --bf-size: jfgpu_params.bf_size of a shard engine is the GLOBAL expected number of k-mers; each shard keeps a
+ *    filter sized for ceil(bf_size / n_shards) of them (bloom_setup: bits and hash count as for one filter) in front of its
+ *    own part of the table.  filter_bf (count_main.cc:122-133) drops the first occurrence of a k-mer, which needs one filter
+ *    to see every occurrence: jfgpu_extract_route routes unfiltered and jfgpu_insert_keys applies the filter on the owner.
+ *    The record exchange (jfgpu_shard_*) takes neither: jfgpu_shard_setup declines an engine with a Bloom structure and
+ *    jfgpu_shard_extract returns JFGPU_ERR_STATE for one.
+ *    `bc` across ranks: every rank builds a counter of its own text (bloom_counter = 1, the same k, size and fpr everywhere,
+ *    so m, nb_hashes and both matrices agree).  A position of the counter is a saturating count min(2, hits)
+ *    (bloom_counter2.hpp:56-107) held as two bits, (hit, hit again); combining two counters is order-independent:
+ *    hit = hit_a | hit_b, again = again_a | again_b | (hit_a & hit_b). */
+/* The counter's device words, read-only: ceil(m / 16) uint32, position p at bits 2*(p % 16) (hit) and 2*(p % 16) + 1 (hit
+ * again) of word p / 16; positions >= m are 0.  Drains the engine's work first.  JFGPU_ERR_STATE: not a Bloom counter. */
+int  jfgpu_bloom_words(jfgpu_handle h, void** dev_words, uint64_t* n_words);
+/* Fold another counter of the same m, nb_hashes and matrices into this one: dev_words (device memory, n_words uint32 of
+ * the layout above) are combined with words [first_word, first_word + n_words).  Stream-ordered on `stream` (NULL = the
+ * engine's own stream): the caller synchronises it before reading or dumping the counter. */
+int  jfgpu_bloom_fold(jfgpu_handle h, const void* dev_words, uint64_t first_word, uint64_t n_words, void* stream);
+/* Bytes [first_byte, first_byte + n_bytes) of the file body bloom_base::write_bits writes (five base-3 digits per byte,
+ * bloom_counter2.hpp:34-36; bc_main.cc:139).  first_byte must be a multiple of 16 (80 positions, 5 words), so that a range
+ * starts on a word; the body has ceil(m / 5) bytes. */
+int  jfgpu_bloom_dump_range(jfgpu_handle h, uint64_t first_byte, uint64_t n_bytes, jfgpu_sink_fn sink, void* ctx);
 
 /* -- helpers ------------------------------------------------------------------------ */
 /* The hash matrix the reference would draw as its (skip+1)-th matrix for a table of

@@ -17,7 +17,7 @@ SYMBOLS = [
     "jfgpu_table_info_get", "jfgpu_dump", "jfgpu_lookup", "jfgpu_histogram",
     "jfgpu_reference_matrix", "jfgpu_synth_fasta_bytes", "jfgpu_synth_fasta_device",
     "jfgpu_host_alloc", "jfgpu_host_free", "jfgpu_memcpy_h2d", "jfgpu_kernel_launches", "jfgpu_version",
-    "jfgpu_bloom_info_get", "jfgpu_bloom_load", "jfgpu_bloom_dump",
+    "jfgpu_bloom_info_get", "jfgpu_bloom_load", "jfgpu_bloom_dump", "jfgpu_bloom_words", "jfgpu_bloom_fold", "jfgpu_bloom_dump_range",
     "jfgpu_set_spill", "jfgpu_shard_setup", "jfgpu_shard_round_bytes", "jfgpu_shard_extract", "jfgpu_shard_pack", "jfgpu_shard_unpack",
     "jfgpu_load_records", "jfgpu_query", "jfgpu_device_count",
 ]
@@ -139,6 +139,12 @@ def load():
     lib.jfgpu_bloom_load.restype = C.c_int
     lib.jfgpu_bloom_dump.argtypes = [H, SINK_FN, C.c_void_p]
     lib.jfgpu_bloom_dump.restype = C.c_int
+    lib.jfgpu_bloom_words.argtypes = [H, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
+    lib.jfgpu_bloom_words.restype = C.c_int
+    lib.jfgpu_bloom_fold.argtypes = [H, C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p]
+    lib.jfgpu_bloom_fold.restype = C.c_int
+    lib.jfgpu_bloom_dump_range.argtypes = [H, C.c_uint64, C.c_uint64, SINK_FN, C.c_void_p]
+    lib.jfgpu_bloom_dump_range.restype = C.c_int
     lib.jfgpu_set_spill.argtypes = [H, SPILL_FN, C.c_void_p]
     lib.jfgpu_set_spill.restype = C.c_int
     lib.jfgpu_shard_setup.argtypes = [H, C.POINTER(ShardBuffers)]

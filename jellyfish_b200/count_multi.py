@@ -10,6 +10,10 @@ byte-identical to what one GPU (or the reference) writes for the same input, sin
 exactly the positions r*size/N ... (r+1)*size/N - 1.  (`jellyfish merge` on the shard files gives the
 same records: jellyfish/merge_files.cc:45-176.)  -m takes 1..128; k > 64 (32-byte keys) is routed by the key exchange
 on 2, 4 or 8 GPUs, with 64 MB batches.
+
+Bloom structures (k <= 64) take the key exchange: `--bc FILE` is loaded whole by every rank and tested before a k-mer is
+routed; `--bf-size N` (the GLOBAL expected number of k-mers) gives every rank a filter for its share, applied by the
+owner after the exchange, where every occurrence of a k-mer arrives.
 """
 import argparse
 import os
@@ -37,9 +41,19 @@ def main(argv=None):
     ap.add_argument("-L", "--lower-count", type=int, default=0)
     ap.add_argument("-U", "--upper-count", type=int, default=(1 << 64) - 1)
     ap.add_argument("-o", "--output", default="mer_counts.jf")
+    ap.add_argument("--bf-size", type=_size, default=0, help="Bloom prefilter: expected number of k-mers (GLOBAL)")
+    ap.add_argument("--bf-fp", type=float, default=0.01, help="false positive rate of the Bloom prefilter")
+    ap.add_argument("--bc", help="count only the k-mers this Bloom counter (written by `bc`) holds twice")
     ap.add_argument("--keep-shards", action="store_true")
     ap.add_argument("files", nargs="+")
     a = ap.parse_args(argv)
+    # the single-GPU command's checks (count_main.cc:196-197 and the k <= 64 scope of every Bloom structure)
+    if a.bf_size and a.bc:
+        sys.stderr.write("Error: Switches [--bf-size] and [--bc] conflict\n")
+        sys.exit(1)
+    if a.mer_len > 64 and (a.bf_size or a.bc):
+        sys.stderr.write("Error: --bf-size and --bc take mer lengths up to 64\n")
+        sys.exit(1)
 
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", rank))
@@ -49,7 +63,7 @@ def main(argv=None):
         os.environ.setdefault("NCCL_MAX_CTAS", "16")      # K1 leaves 16 SMs to the exchange that runs beside it
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     sc = ShardedCounter(a.size, a.counter_len, k=a.mer_len, canonical=a.canonical, rank=rank, world=world, device=local,
-                        reprobes=a.reprobes)
+                        reprobes=a.reprobes, bf_size=a.bf_size, bf_fp=a.bf_fp, bc=a.bc)
     mine = a.files[rank::world]
     rounds = torch.tensor([len(mine)], device="cuda")
     if world > 1:

@@ -21,6 +21,7 @@
 #include "jf_shard.cuh"
 #include "jf_query.cuh"
 #include "jf_wide.cuh"
+#include "jf_bloom.cuh"
 
 using namespace jfk;
 
@@ -425,6 +426,26 @@ const WideKernels& wide_kernels() {
   return w;
 }
 size_t wide_extract_smem(size_t lut_bytes) { return jfw::extract_smem(lut_bytes); }
+
+// The kernels of sharded Bloom counting, compiled in jf_bloom.cu (jf_bloom.cuh), with their types
+struct BloomKernels {
+  void (*insert_keys[5])(TableDev, const uint64_t*, uint32_t, const uint64_t*, uint64_t, BloomDev);   // dispatch order
+  void (*stage_keys[2])(TableDev, PartDev, const uint64_t*, uint32_t, const uint64_t*, uint64_t, BloomDev);
+  void (*fold)(uint32_t*, const uint32_t*, uint64_t);
+};
+const BloomKernels& bloom_kernels() {
+  static const BloomKernels b = [] {
+    const jfbl::Kernels& p = jfbl::kernels();
+    BloomKernels k;
+    for(int i = 0; i < 5; ++i) wide_cast(k.insert_keys[i], p.insert_keys[i]);
+    for(int i = 0; i < 2; ++i) wide_cast(k.stage_keys[i], p.stage_keys[i]);
+    wide_cast(k.fold, p.fold);
+    return k;
+  }();
+  return b;
+}
+// index of insert_keys_bf_kernel<KW, SB> in BloomKernels::insert_keys
+template<int KW, int SB> constexpr int bloom_insert_index() { return KW == 1 ? (SB == 32 ? 0 : SB == 64 ? 1 : 2) : (SB == 64 ? 3 : 4); }
 
 template<int NTH>
 size_t count_smem_bytes(size_t lut_bytes, size_t stage_bytes, size_t bloom_bytes = 0, bool fast = false) {
@@ -967,6 +988,9 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
   a.k = e->k; a.canonical = e->p.canonical; a.nbytes = e->nbytes; a.mode = use; a.format = (uint32_t)e->format;
   a.T = table_dev(e, e->tab);
   a.bloom = bloom_dev(e);
+  // a shard's --bf-size prefilter sees every occurrence of its keys only on the owner (jfgpu_insert_keys): the sender
+  // routes them unfiltered.  (A loaded counter, --bc, is a fixed read-only test: the sender applies it.)
+  if(use == K1_ROUTE && a.bloom.mode == BLOOM_FILTER) memset(&a.bloom, 0, sizeof(a.bloom));
   const size_t bloom_smem = a.bloom.mode ? (size_t)e->nbytes * 256 * 8 * 2 : 0;
   if(bc_build) { a.lut = nullptr; a.lut_bytes = 0; a.hash_fast = 0; }
   a.route_keys = route_keys; a.route_counts = route_counts; a.route_cap = route_cap; a.shard_bits = e->shard_bits;
@@ -1471,8 +1495,9 @@ int jfgpu_create(const jfgpu_params* params, jfgpu_handle* out) {
   if(rc) return bail(rc);
   part_configure(e);
   // count --bf-size: mer_dna_bloom_filter(bf_fp, bf_size) in front of the table (count_main.cc:317-321); its matrices are
-  // drawn when the first unprimed text arrives
-  if(params->bf_size) { rc = bloom_setup(e, BLOOM_FILTER, params->bf_size, params->bf_fp); if(rc) return bail(rc); }
+  // drawn when the first unprimed text arrives.  A shard's filter holds the keys it owns, about 1/n_shards of them: it is
+  // sized for that share of the expected number, so its false positive rate is that of the single filter.
+  if(params->bf_size) { rc = bloom_setup(e, BLOOM_FILTER, (params->bf_size + ns - 1) / ns, params->bf_fp); if(rc) return bail(rc); }
   rc = table_zero(e, e->tab, lazy_zero_ok(e));
   if(rc) return bail(rc);
   rc = reset_carry(e, e->cs);
@@ -1651,7 +1676,7 @@ int jfgpu_feed(jfgpu_handle e, const char* bytes, size_t n, uint32_t flags) {
 int jfgpu_extract_route(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_t flags, void* dev_keys, uint64_t capacity,
                         uint64_t* dev_counts, void* stream) {
   if(!e) return JFGPU_ERR_ARG;
-  if(!e->tab.slots.p || e->bloom.mode != BLOOM_NONE) return fail(e, JFGPU_ERR_STATE, "Bloom filters are not supported on the sharded path");
+  if(!e->tab.slots.p) return fail(e, JFGPU_ERR_STATE, "this engine holds a Bloom counter, not a hash table");
   if(((uintptr_t)dev_bytes & 15) != 0) return fail(e, JFGPU_ERR_ARG, "device text must be 16-byte aligned");
   if(e->kw == 4 && ((uintptr_t)dev_keys & 15) != 0) return fail(e, JFGPU_ERR_ARG, "route buckets of four-word keys must be 16-byte aligned");
   cudaSetDevice(e->device);
@@ -1726,6 +1751,8 @@ uint64_t jfgpu_shard_round_bytes(jfgpu_handle e) {
 int jfgpu_shard_extract(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_t flags, uint32_t bank, void* stream) {
   if(!e) return JFGPU_ERR_ARG;
   if(!e->sh.on || bank > 1) return fail(e, JFGPU_ERR_STATE, "jfgpu_shard_setup has not been called");
+  // the record exchange's send kernels apply no Bloom structure: one attached after jfgpu_shard_setup would be ignored
+  if(e->bloom.mode != BLOOM_NONE) return fail(e, JFGPU_ERR_STATE, "the record exchange takes no Bloom filter (use the key exchange)");
   if(((uintptr_t)dev_bytes & 15) != 0) return fail(e, JFGPU_ERR_ARG, "device text must be 16-byte aligned");
   cudaSetDevice(e->device);
   cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
@@ -1807,6 +1834,11 @@ int jfgpu_insert_keys(jfgpu_handle e, const void* dev_keys, uint64_t n, void* st
   if(n == 0) return JFGPU_OK;
   if(!stream) cudaEventRecord(e->ev_t0, st);
   int rc = JFGPU_OK;
+  // --bf-size on a shard: the prefilter runs here, on the owner, where every occurrence of a key arrives (K1 routes them
+  // unfiltered, run_batch).  Its matrices are the same draws as on every other shard, also when this one has routed nothing.
+  if(e->bloom.mode == BLOOM_FILTER && !e->bloom.drawn && e->op != JFGPU_OP_PRIME) { rc = bloom_draw(e); if(rc) return rc; }
+  const BloomDev bf = e->bloom.mode == BLOOM_FILTER ? bloom_dev(e) : BloomDev();
+  const size_t bf_smem = bf.mode ? (size_t)e->nbytes * 256 * 8 * 2 : 0;
   PartState& ps = e->part;
   if(ps.P) {
     // region-by-region mode: turn the keys into records of the pool (K1c); K2 inserts them at the next drain
@@ -1816,7 +1848,32 @@ int jfgpu_insert_keys(jfgpu_handle e, const void* dev_keys, uint64_t n, void* st
     rc = part_reserve(e, st, chunks_for(ps, per_cta), "record pool smaller than one batch of keys");
     if(rc) return rc;
   }
-  if(ps.P) {
+  if(ps.P && bf.mode) {
+    PartDev pd = part_dev(e);
+    TableDev T = table_dev(e, e->tab);
+    const size_t smem = (size_t)e->nbytes * 256 * 8 + PMAX * 8 + bf_smem;
+    const int grid = (int)std::min<uint64_t>((n + 1024ull * 32 - 1) / (1024ull * 32), (uint64_t)e->n_sm);
+    auto kern = bloom_kernels().stage_keys[e->kw - 1];
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    kern<<<grid, 1024, smem, st>>>(T, pd, e->tab.lut.as<uint64_t>(), e->nbytes, (const uint64_t*)dev_keys, n, bf);
+    JF_LAUNCHED();
+    CUDA_OK(e, cudaGetLastError());
+  } else if(bf.mode) {
+    rc = table_materialize(e, e->tab, st);
+    if(rc) return rc;
+    TableDev T = table_dev(e, e->tab);
+    const size_t smem = (size_t)e->nbytes * 256 * 8 + bf_smem;
+    const int grid = (int)std::min<uint64_t>((n + 255) / 256, (uint64_t)e->n_sm * 8);
+    rc = dispatch(e, e->kw, e->tab.slot_bits, [&](auto KW, auto SB) -> int {
+      auto kern = bloom_kernels().insert_keys[bloom_insert_index<decltype(KW)::value, decltype(SB)::value>()];
+      cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      kern<<<grid, 256, smem, st>>>(T, e->tab.lut.as<uint64_t>(), e->nbytes, (const uint64_t*)dev_keys, n, bf);
+      return JFGPU_OK;
+    });
+    if(rc) return rc;
+    JF_LAUNCHED();
+    CUDA_OK(e, cudaGetLastError());
+  } else if(ps.P) {
     PartDev pd = part_dev(e);
     TableDev T = table_dev(e, e->tab);
     const size_t smem = (size_t)e->nbytes * 256 * 8 + PMAX * 8;
@@ -2290,19 +2347,47 @@ int jfgpu_bloom_load(jfgpu_handle e, uint64_t m, uint32_t nb_hashes, const uint6
   return bloom_upload_matrices(e);
 }
 
-int jfgpu_bloom_dump(jfgpu_handle e, jfgpu_sink_fn sink, void* ctx) {
+int jfgpu_bloom_words(jfgpu_handle e, void** dev_words, uint64_t* n_words) {
+  if(!e || !dev_words || !n_words) return JFGPU_ERR_ARG;
+  cudaSetDevice(e->device);
+  const BloomState& b = e->bloom;
+  if(b.mode != BLOOM_COUNT) return fail(e, JFGPU_ERR_STATE, "no Bloom counter has been built by this engine");
+  int rc = jfgpu_finish(e, nullptr);           // (the words are complete for the caller's streams)
+  if(rc) return rc;
+  *dev_words = b.bits.p; *n_words = b.n_words;
+  return JFGPU_OK;
+}
+
+int jfgpu_bloom_fold(jfgpu_handle e, const void* dev_words, uint64_t first_word, uint64_t n_words, void* stream) {
+  if(!e || (!dev_words && n_words)) return JFGPU_ERR_ARG;
+  cudaSetDevice(e->device);
+  const BloomState& b = e->bloom;
+  if(b.mode != BLOOM_COUNT) return fail(e, JFGPU_ERR_STATE, "no Bloom counter has been built by this engine");
+  if(first_word > b.n_words || n_words > b.n_words - first_word) return fail(e, JFGPU_ERR_ARG, "word range outside the Bloom counter");
+  if(n_words == 0) return JFGPU_OK;
+  cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
+  const int grid = (int)std::min<uint64_t>((n_words + 255) / 256, (uint64_t)e->n_sm * 16);
+  bloom_kernels().fold<<<grid, 256, 0, st>>>(b.bits.as<uint32_t>() + first_word, (const uint32_t*)dev_words, n_words); JF_LAUNCHED();
+  CUDA_OK(e, cudaGetLastError());
+  return JFGPU_OK;
+}
+
+int jfgpu_bloom_dump_range(jfgpu_handle e, uint64_t first_byte, uint64_t n_bytes, jfgpu_sink_fn sink, void* ctx) {
   if(!e || !sink) return JFGPU_ERR_ARG;
   cudaSetDevice(e->device);
   BloomState& b = e->bloom;
   if(b.mode != BLOOM_COUNT) return fail(e, JFGPU_ERR_STATE, "no Bloom counter has been built by this engine");
+  const uint64_t nb = b.m / 5 + (b.m % 5 != 0);
+  if(first_byte % 16 != 0) return fail(e, JFGPU_ERR_ARG, "the first byte of a Bloom counter range must be a multiple of 16");
+  if(first_byte > nb || n_bytes > nb - first_byte) return fail(e, JFGPU_ERR_ARG, "byte range outside the Bloom counter");
   int rc = jfgpu_finish(e, nullptr);
   if(rc) return rc;
-  const uint64_t nb = b.m / 5 + (b.m % 5 != 0);
   const uint64_t piece = (uint64_t)64 << 20;
   DevBuf out; HostBuf<uint8_t> hbuf;
   if(make_all(need(out, piece), need(hbuf, piece)) != cudaSuccess) return fail(e, JFGPU_ERR_NOMEM, "allocation of the Bloom counter staging buffers failed");
-  for(uint64_t off = 0; off < nb && !rc; off += piece) {
-    const uint64_t len = std::min(piece, nb - off);
+  const uint64_t end = first_byte + n_bytes;
+  for(uint64_t off = first_byte; off < end && !rc; off += piece) {
+    const uint64_t len = std::min(piece, end - off);
     const int grid = (int)std::min<uint64_t>((len + 255) / 256, (uint64_t)e->n_sm * 16);
     // positions 5*off .. : the kernel takes the bit array shifted by whole words (5*off*2 bits; piece is a multiple of 16 bytes)
     bloom_pack_kernel<<<grid, 256, 0, e->cs>>>(b.bits.as<uint32_t>() + (5 * off) / 16, b.m - 5 * off, len, out.as<uint8_t>()); JF_LAUNCHED();
@@ -2312,6 +2397,12 @@ int jfgpu_bloom_dump(jfgpu_handle e, jfgpu_sink_fn sink, void* ctx) {
     if(sink(ctx, hbuf, len) != 0) rc = fail(e, JFGPU_ERR_SINK, "dump sink failed");
   }
   return rc;
+}
+
+int jfgpu_bloom_dump(jfgpu_handle e, jfgpu_sink_fn sink, void* ctx) {
+  if(!e || !sink) return JFGPU_ERR_ARG;
+  if(e->bloom.mode != BLOOM_COUNT) return fail(e, JFGPU_ERR_STATE, "no Bloom counter has been built by this engine");
+  return jfgpu_bloom_dump_range(e, 0, e->bloom.m / 5 + (e->bloom.m % 5 != 0), sink, ctx);
 }
 
 uint64_t jfgpu_synth_fasta_bytes(uint64_t n_bases) {

@@ -555,15 +555,22 @@ __global__ void __launch_bounds__(512, 2) insert_chunks_kernel(TableDev T, PartD
 // K1c: packed keys -> records appended to the per-CTA chunk lists (the receive side of the
 //      multi-GPU all-to-all in region-by-region mode: same record pool, same K2 afterwards).
 // ---------------------------------------------------------------------------------------
-template<int KW>
-__global__ void __launch_bounds__(1024, 1) stage_keys_kernel(TableDev T, PartDev pd, const uint64_t* __restrict__ lut_g, uint32_t nbytes,
-                                                              const uint64_t* __restrict__ keys, uint64_t n, uint64_t* __restrict__ spill_keys_unused) {
+// BF: the --bf-size prefilter of a shard in front of the table, as in insert_keys_bf_kernel; its byte tables follow the
+// staging counters in shared memory.  (stage_keys_bf_kernel is instantiated in jf_bloom.cu only.)
+template<int KW, bool BF>
+__device__ __forceinline__ void stage_keys_body(const TableDev& T, const PartDev& pd, const uint64_t* __restrict__ lut_g, uint32_t nbytes,
+                                                const uint64_t* __restrict__ keys, uint64_t n, const BloomDev& B) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   uint64_t* lut = reinterpret_cast<uint64_t*>(smem_raw);
   uint32_t* st_cnt = reinterpret_cast<uint32_t*>(lut + nbytes * 256);
   uint32_t* st_chunk = st_cnt + PMAX;
+  uint64_t* bl1 = reinterpret_cast<uint64_t*>(st_chunk + PMAX);
+  uint64_t* bl2 = bl1 + nbytes * 256;
   const int tid = threadIdx.x;
-  for(uint32_t i = tid; i < nbytes * 256u; i += blockDim.x) lut[i] = lut_g[i];
+  for(uint32_t i = tid; i < nbytes * 256u; i += blockDim.x) {
+    lut[i] = lut_g[i];
+    if constexpr(BF) { bl1[i] = B.lut1[i]; bl2[i] = B.lut2[i]; }
+  }
   uint32_t* my_chunk = pd.cta_chunk + (size_t)blockIdx.x * pd.P;
   uint32_t* my_fill  = pd.cta_fill + (size_t)blockIdx.x * pd.P;
   for(uint32_t p = tid; p < pd.P; p += blockDim.x) {
@@ -584,6 +591,9 @@ __global__ void __launch_bounds__(1024, 1) stage_keys_kernel(TableDev T, PartDev
       uint64_t key[KW];
 #pragma unroll
       for(int w = 0; w < KW; ++w) key[w] = keys[i * KW + w];
+      if constexpr(BF) {
+        if(!bloom_test_and_set(B, gf2_hash<KW>(bl1, key, (int)nbytes), gf2_hash<KW>(bl2, key, (int)nbytes))) continue;
+      }
       const uint64_t pos = gf2_hash<KW>(lut, key, (int)nbytes);
       const uint64_t lpos = pos & T.local_mask;
       const uint32_t p = (uint32_t)(lpos >> pd.region_bits);
@@ -605,6 +615,16 @@ __global__ void __launch_bounds__(1024, 1) stage_keys_kernel(TableDev T, PartDev
     __syncthreads();
   }
   for(uint32_t p = tid; p < pd.P; p += blockDim.x) { my_chunk[p] = st_chunk[p]; my_fill[p] = min(st_cnt[p], pd.chunk_recs); }
+}
+template<int KW>
+__global__ void __launch_bounds__(1024, 1) stage_keys_kernel(TableDev T, PartDev pd, const uint64_t* __restrict__ lut_g, uint32_t nbytes,
+                                                              const uint64_t* __restrict__ keys, uint64_t n, uint64_t* __restrict__ spill_keys_unused) {
+  stage_keys_body<KW, false>(T, pd, lut_g, nbytes, keys, n, BloomDev());
+}
+template<int KW>
+__global__ void __launch_bounds__(1024, 1) stage_keys_bf_kernel(TableDev T, PartDev pd, const uint64_t* __restrict__ lut_g, uint32_t nbytes,
+                                                                 const uint64_t* __restrict__ keys, uint64_t n, BloomDev B) {
+  stage_keys_body<KW, true>(T, pd, lut_g, nbytes, keys, n, B);
 }
 
 // ---- lean specialisation of K2 for the common geometry: 32-bit slots and 4-byte records ----
@@ -820,6 +840,32 @@ __global__ void __launch_bounds__(256) insert_keys_kernel(TableDev T, const uint
     const uint64_t pos = gf2_hash<KW>(lut, key, (int)nbytes);
     if(table_add<KW, SB>(T, key, pos, cnt, ls)) occ += cnt;
     else { ls.failed++; record_failure<KW>(T, key, cnt); }
+  }
+  flush_stats(T.stats, occ, ls.distinct, ls.reprobes);
+}
+// The same with the --bf-size prefilter of a shard in front of the table (sharded counting applies it on the owner, where
+// every occurrence of a key arrives; jfgpu_insert_keys): a key reaches the table only when the filter has seen it before.
+// The filter's two byte tables follow the table's in shared memory.  (A kernel of its own rather than a template switch of
+// the one above, whose code stays as it was; instantiated in jf_bloom.cu only.)
+template<int KW, int SB>
+__global__ void __launch_bounds__(256) insert_keys_bf_kernel(TableDev T, const uint64_t* __restrict__ lut_g, uint32_t nbytes,
+                                                             const uint64_t* __restrict__ keys, uint64_t n, BloomDev B) {
+  extern __shared__ __align__(16) uint8_t smem_raw[];
+  uint64_t* lut = reinterpret_cast<uint64_t*>(smem_raw);
+  uint64_t* bl1 = lut + nbytes * 256;
+  uint64_t* bl2 = bl1 + nbytes * 256;
+  for(uint32_t i = threadIdx.x; i < nbytes * 256u; i += blockDim.x) { lut[i] = lut_g[i]; bl1[i] = B.lut1[i]; bl2[i] = B.lut2[i]; }
+  __syncthreads();
+  LocalStats ls = { 0, 0, 0, 0, 0 };
+  unsigned long long occ = 0;
+  for(uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    uint64_t key[KW];
+#pragma unroll
+    for(int q = 0; q < KW; ++q) key[q] = keys[i * KW + q];
+    if(!bloom_test_and_set(B, gf2_hash<KW>(bl1, key, (int)nbytes), gf2_hash<KW>(bl2, key, (int)nbytes))) continue;
+    const uint64_t pos = gf2_hash<KW>(lut, key, (int)nbytes);
+    if(table_add<KW, SB>(T, key, pos, 1, ls)) occ++;
+    else { ls.failed++; record_failure<KW>(T, key, 1); }
   }
   flush_stats(T.stats, occ, ls.distinct, ls.reprobes);
 }

@@ -214,16 +214,27 @@ def default_batch_bytes(k):
 
 
 class ShardedCounter(object):
-    """hash_counter over `world` GPUs.  `size` is the GLOBAL table size (jellyfish count -s)."""
+    """hash_counter over `world` GPUs.  `size` is the GLOBAL table size (jellyfish count -s).
+
+    Bloom structures (k <= 64): `bf_size` (count --bf-size, the GLOBAL expected number of k-mers; `bf_fp` its false positive
+    rate) puts a prefilter in front of every shard, applied by the owner after the exchange; `bc` (count --bc) is the path of
+    a counter written by `jellyfish bc`, loaded whole by every rank and applied by the sender before the exchange.  Both take
+    the key exchange: the record exchange applies no filter."""
 
     def __init__(self, size, val_len=7, k=None, canonical=False, rank=0, world=1, device=0, reprobes=126,
-                 batch_bytes=None, slack=1.25, exchange="auto", send_gb=None, **engine_kw):
+                 batch_bytes=None, slack=1.25, exchange="auto", send_gb=None, bf_size=0, bf_fp=0.0, bc=None, **engine_kw):
         from .engine import HashCounter
+        if bf_size and bc:
+            raise ValueError("Switches [--bf-size] and [--bc] conflict")
         if batch_bytes is None:
             batch_bytes = default_batch_bytes(k)
         self.rank, self.world = rank, world
         self.hc = HashCounter(size, val_len, k=k, canonical=canonical, reprobes=reprobes, device=device,
-                              shard_index=rank, n_shards=world, allow_regrow=(world == 1), max_batch_bytes=batch_bytes, **engine_kw)
+                              shard_index=rank, n_shards=world, allow_regrow=(world == 1), max_batch_bytes=batch_bytes,
+                              bf_size=bf_size, bf_fp=bf_fp, **engine_kw)
+        if bc:
+            # before the exchange form is chosen: the record exchange declines an engine with a Bloom structure
+            self.hc.load_bloom_counter(bc)
         self.backend = EngineBackend(self.hc)
         self.batch_bytes = batch_bytes
         self.dev = torch.device("cuda", device)
@@ -341,6 +352,152 @@ class ShardedCounter(object):
     def dump_shard(self, path, **kw):
         """Every rank writes `path.<rank>`: header (global size/matrix) + its sorted records."""
         return self.hc.dump("%s.%d" % (path, self.rank), **kw)
+
+
+class BloomBackend(object):
+    """What the combination of Bloom counters across ranks needs from the engine; the CUDA engine implements it with kernels.
+    A counter is n_words 32-bit words (16 positions each, two bits a position: hit, hit again) whose file body has n_bytes
+    bytes (five positions a byte)."""
+
+    n_words = n_bytes = 0
+
+    def words(self):
+        """int32 tensor of the counter's n_words words (read-only; on the device of the exchange)"""
+        raise NotImplementedError
+
+    def fold(self, words, first_word):
+        """fold an int32 tensor of another counter's words into words [first_word, first_word + len(words))"""
+        raise NotImplementedError
+
+    def dump_range(self, first_byte, n_bytes, sink):
+        """sink(bytes) with bytes [first_byte, first_byte + n_bytes) of the file body"""
+        raise NotImplementedError
+
+
+class _DeviceWords(object):
+    """A device buffer the engine owns, seen by torch (CUDA array interface)."""
+
+    def __init__(self, ptr, n):
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": "<i4", "data": (ptr, False), "version": 2}
+
+
+class EngineBloomBackend(BloomBackend):
+    """libjfgpu.so behind the seam: jfgpu_bloom_words / jfgpu_bloom_fold / jfgpu_bloom_dump_range of a BloomCounter."""
+
+    def __init__(self, bc, dev):
+        self.bc, self.dev = bc, dev
+
+    def words(self):
+        ptr, self.n_words = self.bc.words()
+        self.n_bytes = self.bc.info()["nb_bytes"]
+        return torch.as_tensor(_DeviceWords(ptr, self.n_words), device=self.dev)
+
+    def fold(self, words, first_word):
+        # on torch's current stream, behind the collective that delivered the words
+        self.bc.fold(words.data_ptr(), first_word, words.numel(), stream=torch.cuda.current_stream(self.dev).cuda_stream)
+
+    def dump_range(self, first_byte, n_bytes, sink):
+        torch.cuda.current_stream(self.dev).synchronize()     # every fold is done
+        self.bc.dump_range(first_byte, n_bytes, sink)
+
+
+def bloom_slices(n_words, world):
+    """[first_word, end_word) of every rank's slice of a counter: boundaries on the 5-word grid (80 positions, 16 bytes of
+    the file body), the last slice ends at n_words."""
+    units = (n_words + 4) // 5
+    return [(min(5 * (units * r // world), n_words), min(5 * (units * (r + 1) // world), n_words)) for r in range(world)]
+
+
+def bloom_byte_range(first_word, end_word, n_words, n_bytes):
+    """The bytes of the file body that words [first_word, end_word) of a slice hold."""
+    def to_byte(w):
+        return n_bytes if w >= n_words else w // 5 * 16
+    return to_byte(first_word), to_byte(end_word)
+
+
+def bloom_reduce_scatter(backend, rank, world, piece_words=64 << 20):
+    """Fold every rank's counter into the slice this rank owns (bloom_slices): a reduce-scatter made of all-to-alls of at
+    most `piece_words` words per peer, so that it takes world * piece_words words of extra memory (256 MB per peer by
+    default) rather than a second counter.  Returns this rank's (first_word, end_word)."""
+    words = backend.words()
+    sl = bloom_slices(words.numel(), world)
+    longest = max(e - b for b, e in sl)
+    pw = max(1, min(piece_words, longest))
+    recv = torch.empty((world, pw), dtype=torch.int32, device=words.device)
+    me0 = sl[rank][0]
+    for p in range((longest + pw - 1) // pw):
+        off = p * pw
+        lens = [max(0, min(pw, e - b - off)) for b, e in sl]
+        # this rank's own piece does not travel
+        ins = [words[b + off:b + off + (0 if d == rank else lens[d])] for d, (b, e) in enumerate(sl)]
+        rl = [0 if s == rank else lens[rank] for s in range(world)]
+        outs = [recv[s, :rl[s]] for s in range(world)]
+        if dist.get_backend() == "nccl":
+            dist.all_to_all(outs, ins)
+        else:
+            flat = torch.empty(sum(rl), dtype=torch.int32, device=words.device)
+            dist.all_to_all_single(flat, torch.cat(ins), output_split_sizes=rl, input_split_sizes=[x.numel() for x in ins])
+            o = 0
+            for s in range(world):
+                outs[s].copy_(flat[o:o + rl[s]])
+                o += rl[s]
+        for s in range(world):
+            if rl[s]:
+                backend.fold(outs[s], me0 + off)
+    return sl[rank]
+
+
+class ShardedBloomCounter(object):
+    """`jellyfish bc` over `world` GPUs (bc_main.cc:84-161): every rank builds a counter of its own text with the same k,
+    size and false positive rate (so the same m, nb_hashes and matrices: the first draws of the reference's stream), then
+    the counters are folded into one, rank r holding slice r (bloom_reduce_scatter), and every rank writes the bytes of its
+    slice.  The combination is independent of the order of the hits, so the rank-ordered concatenation is the file one GPU
+    (or the reference) writes for all the text."""
+
+    def __init__(self, size, fpr=0.001, k=None, canonical=False, rank=0, world=1, device=0, piece_bytes=256 << 20):
+        from .engine import BloomCounter
+        self.rank, self.world = rank, world
+        self.dev = torch.device("cuda", device)
+        self.bc = BloomCounter(size, fpr, k=k, canonical=canonical, device=device)
+        self.backend = EngineBloomBackend(self.bc, self.dev)
+        self.piece_words = max(1, piece_bytes // 4)
+
+    def add_files(self, paths):
+        self.bc.add_files(paths)
+
+    def combine(self):
+        """-> (first_byte, n_bytes) of the file body this rank holds once every counter is folded in"""
+        if self.world == 1:
+            return 0, self.bc.info()["nb_bytes"]
+        b, e = bloom_reduce_scatter(self.backend, self.rank, self.world, self.piece_words)
+        first, end = bloom_byte_range(b, e, self.backend.n_words, self.backend.n_bytes)
+        return first, end - first
+
+    def dump_slice(self, path):
+        """combine(), then `path.<rank>`: the body bytes of this rank's slice (no header)"""
+        first, n = self.combine()
+        out = "%s.%d" % (path, self.rank)
+        with open(out, "wb") as f:
+            self.backend.dump_range(first, n, f.write)
+        return out
+
+    def header(self, cmdline=()):
+        return self.bc.header(cmdline)
+
+    def close(self):
+        self.bc.close()
+
+
+def concat_bloom_slices(path, world, header, out=None):
+    """header + the rank-ordered concatenation of the slice files `path.<rank>` (ShardedBloomCounter.dump_slice)."""
+    from .engine import write_header
+    out = out or path
+    with open(out, "wb") as fo:
+        write_header(fo, header)
+        for r in range(world):
+            with open("%s.%d" % (path, r), "rb") as fi:
+                fo.write(fi.read())
+    return out
 
 
 def concat_shards(path, world, out=None):

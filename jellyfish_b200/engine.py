@@ -408,12 +408,28 @@ class BloomCounter(object):
         """header + filter.write_bits (bc_main.cc:113,139)."""
         with open(path, "wb") as f:
             write_header(f, self.header(cmdline))
+            self.dump_range(0, self.info()["nb_bytes"], f.write)
 
-            def _sink(ctx, ptr, n):
-                f.write(C.string_at(ptr, n))
-                return 0
-            cb = L.SINK_FN(_sink)
-            self.hc._check(self.hc._lib.jfgpu_bloom_dump(self.hc._h, cb, None))
+    # -- combining counters across ranks (include/jfgpu.h: jfgpu_bloom_words / _fold / _dump_range) ------------------------
+    def words(self):
+        """-> (device pointer, number) of the counter's 32-bit words: position p at bits 2*(p % 16) (hit) and 2*(p % 16)+1
+        (hit again) of word p // 16."""
+        ptr, n = C.c_void_p(), C.c_uint64()
+        self.hc._check(self.hc._lib.jfgpu_bloom_words(self.hc._h, C.byref(ptr), C.byref(n)))
+        return ptr.value or 0, n.value
+
+    def fold(self, dev_ptr, first_word, n_words, stream=None):
+        """Fold n_words words of another counter (device memory) into words [first_word, first_word + n_words) of this one
+        (stream-ordered)."""
+        self.hc._check(self.hc._lib.jfgpu_bloom_fold(self.hc._h, C.c_void_p(dev_ptr), first_word, n_words, C.c_void_p(stream or 0)))
+
+    def dump_range(self, first_byte, n_bytes, sink):
+        """sink(bytes) with bytes [first_byte, first_byte + n_bytes) of the file body; first_byte a multiple of 16."""
+        def _sink(ctx, ptr, n):
+            sink(C.string_at(ptr, n))
+            return 0
+        cb = L.SINK_FN(_sink)
+        self.hc._check(self.hc._lib.jfgpu_bloom_dump_range(self.hc._h, first_byte, n_bytes, cb, None))
 
 
 def read_header(path):
