@@ -189,6 +189,7 @@ struct jfgpu_engine {
   size_t batch_bytes = 0;
   DevBuf stage[2]; Event ev_copied[2], ev_done[2];
   int stage_cur = 0;
+  uint8_t stage_look[2] = {0, 0};           // look-ahead byte staged behind a batch that ends in '\r' (run_staged)
   // per-batch scratch
   DevBuf nlA, nlB, cntA, cntB, tstate; uint64_t scratch_tiles = 0;
   int format = 0;                 // 0 = FASTA, 1 = FASTQ: format of the file being fed
@@ -1540,12 +1541,26 @@ static int begin_device_feed(jfgpu_engine* e, uint32_t flags, const void* dev_by
 
 // One batch of host text through the next staging buffer: copied on the copy stream, run on the compute stream once the
 // copy is done.  The caller has waited for ev_done of that buffer (the previous batch that used it has finished).
-static int run_staged(jfgpu_engine* e, const char* bytes, size_t len, K1Use use) {
+// The batch is bytes [off, off + len) of the n bytes of this feed.  A batch that still ends on '\r' (next_batch_len could not
+// cut in front of the run: the run fills the batch, or follows its first byte) gets the byte that ends the run staged behind
+// it as one byte of look-ahead, so that the device drops the run when a '\n' ends it and resets the window when a base does,
+// as it would with the whole text in view.  A run that reaches the end of the data is a line end.
+static int run_staged(jfgpu_engine* e, const char* bytes, size_t off, size_t len, size_t n, K1Use use) {
   const int s = e->stage_cur;
-  CUDA_OK(e, cudaMemcpyAsync(e->stage[s].p, bytes, len, cudaMemcpyHostToDevice, e->hs));
+  CUDA_OK(e, cudaMemcpyAsync(e->stage[s].p, bytes + off, len, cudaMemcpyHostToDevice, e->hs));
+  size_t n_look = len;
+  if(len && off + len < n && bytes[off + len - 1] == '\r') {
+    size_t q = off + len;
+    while(q < n && bytes[q] == '\r') ++q;
+    if(q < n) {
+      e->stage_look[s] = (uint8_t)bytes[q];
+      CUDA_OK(e, cudaMemcpyAsync(e->stage[s].as<uint8_t>() + len, &e->stage_look[s], 1, cudaMemcpyHostToDevice, e->hs));
+      n_look = len + 1;
+    }
+  }
   CUDA_OK(e, cudaEventRecord(e->ev_copied[s], e->hs));
   CUDA_OK(e, cudaStreamWaitEvent(e->cs, e->ev_copied[s], 0));
-  const int rc = run_batch(e, e->stage[s].as<uint8_t>(), len, len, e->cs, use);
+  const int rc = run_batch(e, e->stage[s].as<uint8_t>(), len, n_look, e->cs, use);
   if(rc) return rc;
   CUDA_OK(e, cudaEventRecord(e->ev_done[s], e->cs));
   e->stage_cur ^= 1;
@@ -1609,8 +1624,9 @@ static size_t fastq_record_prefix(const char* p, size_t len, uint32_t lines_mod4
   return best;
 }
 
-// Length of the next batch of host text at `off`, at most `cap` bytes: it never ends on '\r' unless the data ends there (the
-// device looks one byte ahead), and with `qfastq` (-Q on FASTQ) only behind a complete record (e->q_lines follows).
+// Length of the next batch of host text at `off`, at most `cap` bytes: it ends in front of a '\r' run that would end it
+// (the device looks ahead to see where a run ends; when the run fills all but the first byte, run_staged gives it the byte
+// that ends the run), and with `qfastq` (-Q on FASTQ) only behind a complete record (e->q_lines follows).
 static int next_batch_len(jfgpu_engine* e, const char* bytes, size_t off, size_t n, size_t cap, bool qfastq, size_t* out) {
   size_t len = cap;
   if(off + len < n) { size_t l2 = len; while(l2 > 1 && bytes[off + l2 - 1] == '\r') --l2; if(l2 > 1) len = l2; }
@@ -1659,7 +1675,7 @@ int jfgpu_feed(jfgpu_handle e, const char* bytes, size_t n, uint32_t flags) {
       CUDA_OK(e, cudaStreamSynchronize(e->hs));
       if(e->h_stats[STAT_FAILED]) { rc = check_after_batches(e); if(rc) return rc; }
     }
-    rc = run_staged(e, bytes + off, len, K1_COUNT);
+    rc = run_staged(e, bytes, off, len, n, K1_COUNT);
     if(rc) return rc;
     off += len;
   }
@@ -2184,7 +2200,7 @@ static int query_impl(jfgpu_engine* e, const char* bytes, size_t n, uint32_t fla
     jfgpu_engine::QueryBufs& q = e->qb[b];
     CUDA_OK(e, cudaEventSynchronize(e->ev_done[e->stage_cur]));
     e->q_cur = b;
-    int rc2 = run_staged(e, bytes + off, len, K1_QUERY);
+    int rc2 = run_staged(e, bytes, off, len, n, K1_QUERY);
     if(rc2) return rc2;
     q.n_tiles = (len + TILE - 1) / TILE;
     const int grid = (int)std::min<uint64_t>(q.n_tiles, (uint64_t)e->n_sm * 8);
