@@ -38,8 +38,20 @@ enum {
 /* feed flags */
 enum {
   JFGPU_FILE_BEGIN = 1u,  /* first bytes of an input file: format is sniffed here    */
-  JFGPU_FILE_END   = 2u   /* last bytes of an input file: no k-mer spans the file end
+  JFGPU_FILE_END   = 2u,  /* last bytes of an input file: no k-mer spans the file end
                              (mer_overlap_sequence_parser.hpp:111)                  */
+  /* Alignment records (count --sam, mer_overlap_sequence_parser.hpp:220-253).  Given with JFGPU_FILE_BEGIN, the file is read
+   * in that form instead of being sniffed from its first byte, for all its feeds (a later feed may repeat the flag).  Every
+   * record counts as a FASTQ read of its SEQ (ACGT in either case are bases, anything else an N) with its QUAL, FLAG ignored.
+   * SAM: text; lines starting with '@' and blank lines are skipped, one '\r' in front of a '\n' ends the line; a QUAL of
+   *   '*' gives every base the quality character 0x20.  jfgpu_feed and jfgpu_feed_device.
+   * BAM: the INFLATED stream (magic "BAM\1", l_text, text, references, records; little-endian); quality character =
+   *   phred + 33 (mod 256).  jfgpu_feed only.
+   * An incomplete last line, header or record of a feed is carried to the next one.  A malformed record (fewer than 11
+   * fields, SEQ and QUAL of different lengths, a BAM record or header cut short or with a bad magic) fails the feed with
+   * JFGPU_ERR_FORMAT.  jfgpu_query, jfgpu_extract_route and jfgpu_shard_extract take neither flag (JFGPU_ERR_ARG). */
+  JFGPU_FORMAT_SAM = 4u,
+  JFGPU_FORMAT_BAM = 8u
 };
 
 /* operations of mer_counter_base (sub_commands/count_main.cc:133,152-184) */

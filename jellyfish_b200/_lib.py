@@ -24,6 +24,7 @@ SYMBOLS = [
 
 OK, ERR_ARG, ERR_CUDA, ERR_FULL, ERR_FORMAT, ERR_STATE, ERR_NOMEM, ERR_SINK = range(8)
 FILE_BEGIN, FILE_END = 1, 2
+FORMAT_SAM, FORMAT_BAM = 4, 8
 
 
 class Params(C.Structure):

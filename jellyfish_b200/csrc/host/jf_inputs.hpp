@@ -38,6 +38,8 @@
 #include <thread>
 #include <vector>
 
+#include "jf_sam_input.hpp"
+
 extern char** environ;
 
 namespace jfb {
@@ -218,11 +220,14 @@ struct input_buffers {                                   // where the chunks liv
   std::function<void(void*)> release;
 };
 
-// Files first, then the generator outputs, through `feed(data, n, flags)` (non-zero return = stop, its message via
-// feed_error).  A reader thread fills three buffers ahead of the feeding thread.  Returns "" or the error of the run.
+// Files first, then the generator outputs, then the --sam files (stream_manager.hpp:134-145), through `feed(data, n, flags)`
+// (non-zero return = stop, its message via feed_error).  The first chunk of a --sam file carries INPUT_FORMAT_SAM or
+// INPUT_FORMAT_BAM (jf_sam_input.hpp).  A reader thread fills three buffers ahead of the feeding thread.  Returns "" or the
+// error of the run.
 inline std::string stream_inputs(const std::vector<const char*>& files, const generator_spec& gen, const input_buffers& mem,
                                  const std::function<int(const char*, size_t, uint32_t)>& feed,
-                                 const std::function<std::string()>& feed_error, size_t buf_bytes = (size_t)64 << 20) {
+                                 const std::function<std::string()>& feed_error, size_t buf_bytes = (size_t)64 << 20,
+                                 const std::vector<const char*>& sam_files = {}) {
   std::vector<std::string> cmds;
   const char* shell = gen.shell;
   if(gen.given()) {
@@ -244,7 +249,7 @@ inline std::string stream_inputs(const std::vector<const char*>& files, const ge
     auto get_buf = [&]() { std::unique_lock<std::mutex> l(mu); cv.wait(l, [&] { return !freeb.empty(); }); char* b = freeb.front(); freeb.pop(); return b; };
     auto put = [&](chunk c) { std::unique_lock<std::mutex> l(mu); ready.push(c); cv.notify_all(); };
     // one input, read one chunk ahead so that the last chunk can carry FILE_END; `more(dst, n, &err)` = bytes read, 0 at the end
-    auto one_input = [&](const std::function<size_t(char*, size_t, std::string*)>& more) -> std::string {
+    auto one_input = [&](const std::function<size_t(char*, size_t, std::string*)>& more, uint32_t begin = INPUT_FILE_BEGIN) -> std::string {
       bool first = true, eof = false;
       std::string io_error;
       auto fill = [&](char* b) -> size_t {
@@ -267,7 +272,7 @@ inline std::string stream_inputs(const std::vector<const char*>& files, const ge
           return io_error;
         }
         const bool last_of_input = eof && nn == 0;
-        const uint32_t fl = (first ? INPUT_FILE_BEGIN : 0u) | (last_of_input ? INPUT_FILE_END : 0u);
+        const uint32_t fl = (first ? begin : 0u) | (last_of_input ? INPUT_FILE_END : 0u);
         put(chunk{cur, have, fl, false, ""});
         first = false;
         if(last_of_input) { if(nxt) { std::unique_lock<std::mutex> l(mu); freeb.push(nxt); } return ""; }
@@ -311,6 +316,13 @@ inline std::string stream_inputs(const std::vector<const char*>& files, const ge
     running.clear();                                        // (terminates what is still running after a failure)
     if(stop.load()) { put(chunk{nullptr, 0, 0, true, ""}); return; }
     if(!failed.empty()) { put(chunk{nullptr, 0, 0, true, failed + "\nSome generator commands failed"}); return; }
+    for(size_t fi = 0; fi < sam_files.size() && !stop.load(); ++fi) {
+      sam_source src;
+      uint32_t form = 0;
+      std::string err = src.open(sam_files[fi], &form);
+      if(err.empty()) err = one_input([&](char* dst, size_t n, std::string* e) { return src.read(dst, n, e); }, INPUT_FILE_BEGIN | form);
+      if(!err.empty()) { put(chunk{nullptr, 0, 0, true, err}); return; }
+    }
     put(chunk{nullptr, 0, 0, true, ""});
   });
   std::string error;

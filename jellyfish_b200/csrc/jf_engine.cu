@@ -22,6 +22,7 @@
 #include "jf_query.cuh"
 #include "jf_wide.cuh"
 #include "jf_bloom.cuh"
+#include "jf_sam.cuh"
 
 using namespace jfk;
 
@@ -33,6 +34,7 @@ static thread_local std::string g_create_error;
 namespace {
 
 constexpr unsigned SHARD_RESERVED_SMS = 16;
+constexpr uint32_t SAM_FLAGS = JFGPU_FORMAT_SAM | JFGPU_FORMAT_BAM;
 constexpr uint64_t WIN_DEF_CAP = (uint64_t)16 << 20;   // deferred records per group of the window form of K2   // SMs K1 leaves to NCCL while an exchange runs beside it
 
 unsigned ceil_log2(uint64_t x) { unsigned l = 0; while(l < 64 && ((uint64_t)1 << l) < x) ++l; return l; }
@@ -229,6 +231,20 @@ struct jfgpu_engine {
   } qb[2];
   HostBuf<uint8_t> q_host[2]; Event ev_qcopy[2];
   uint64_t q_tiles_cap = 0; int q_cur = 0;
+  // SAM / BAM input (jf_sam.cu): the form of the file being fed (0 = FASTA / FASTQ text, 1 = SAM, 2 = BAM), the buffers of a
+  // batch (made at the first such file; one of each: a batch is transcoded and read back before the next is staged) and what
+  // a feed leaves to the next one
+  struct SamState {
+    uint32_t form = 0;
+    size_t in_cap = 0;                              // input bytes of a batch: its FASTQ, at most twice as long, is one K1 batch
+    DevBuf out, scratch, res, offs, tail_dev;       // FASTQ, kernel scratch, jfsam::Result, BAM record offsets, device carry
+    HostBuf<jfsam::Result> h_res; HostBuf<uint32_t> h_offs;
+    std::string tail;                               // host feeds: the incomplete last line, or the cut BAM header field or record
+    size_t tail_dev_len = 0;                        // device feeds: bytes of the incomplete last line in tail_dev
+    uint32_t bam_phase = 0, bam_refs = 0;           // BAM walk: which header field comes next, references left
+    uint64_t bam_skip = 0;                          // bytes of header text or reference name still to pass over
+    uint64_t done_off = 0;                          // bytes of the file in front of the next batch (messages)
+  } sam;
 };
 
 namespace {
@@ -1517,9 +1533,13 @@ void jfgpu_destroy(jfgpu_handle e) {
 
 static int begin_feed(jfgpu_engine* e, uint32_t flags, int first_byte, cudaStream_t st) {
   if(flags & JFGPU_FILE_BEGIN) {
-    // mer_overlap_sequence_parser.hpp:134-148: the first byte selects the format
-    if(first_byte >= 0 && first_byte != '>' && first_byte != '@') return fail(e, JFGPU_ERR_FORMAT, "Unsupported format");
-    e->format = first_byte == '@' ? 1 : 0;
+    // mer_overlap_sequence_parser.hpp:134-148: the first byte selects the format, unless the caller gives SAM or BAM
+    const uint32_t form = flags & JFGPU_FORMAT_BAM ? 2 : flags & JFGPU_FORMAT_SAM ? 1 : 0;
+    if(!form && first_byte >= 0 && first_byte != '>' && first_byte != '@') return fail(e, JFGPU_ERR_FORMAT, "Unsupported format");
+    // SAM and BAM records reach the extraction kernels as 4-line FASTQ
+    e->format = form || first_byte == '@' ? 1 : 0;
+    e->sam.form = form; e->sam.tail.clear(); e->sam.tail_dev_len = 0;
+    e->sam.bam_phase = 0; e->sam.bam_refs = 0; e->sam.bam_skip = 0; e->sam.done_off = 0;
     int rc = reset_carry(e, st);
     if(rc) return rc;
     e->in_file = true;
@@ -1570,7 +1590,7 @@ static int run_staged(jfgpu_engine* e, const char* bytes, size_t off, size_t len
 static int end_feed(jfgpu_engine* e, uint32_t flags, cudaStream_t st) {
   if(flags & JFGPU_FILE_END) {
     // no k-mer spans two files: mer_overlap_sequence_parser.hpp:111
-    e->format = 0;
+    e->format = 0; e->sam.form = 0;
     int rc = reset_carry(e, st);
     if(rc) return rc;
     e->in_file = false;
@@ -1578,11 +1598,265 @@ static int end_feed(jfgpu_engine* e, uint32_t flags, cudaStream_t st) {
   return JFGPU_OK;
 }
 
+// ---- SAM and BAM input (JFGPU_FORMAT_SAM / _BAM): batches of whole records are rewritten as FASTQ by the kernels of
+// jf_sam.cu and counted as FASTQ.  The FASTQ of a batch is whole records, so the -Q rule "a K1 batch ends on a record
+// boundary" holds by construction.
+enum : uint32_t { BAM_MAGIC = 0, BAM_NREF = 1, BAM_REF = 2, BAM_RECORDS = 3 };
+
+static int sam_alloc(jfgpu_engine* e) {
+  jfgpu_engine::SamState& s = e->sam;
+  if(!e->stage[0].p) CUDA_OK(e, e->stage[0].alloc(e->batch_bytes + 64));
+  if(s.out.p) return JFGPU_OK;
+  s.in_cap = std::max<size_t>(std::min<size_t>(e->batch_bytes / 2, (size_t)1 << 30) & ~(size_t)15, 64);
+  const size_t max_recs = jfsam::max_bam_records(s.in_cap);
+  if(make_all(need(s.out, 2 * s.in_cap + 64), need(s.scratch, jfsam::scratch_bytes(s.in_cap)), need(s.res, sizeof(jfsam::Result)),
+              need(s.offs, max_recs * 4), need(s.tail_dev, s.in_cap + 64), need(s.h_res, sizeof(jfsam::Result)),
+              need(s.h_offs, max_recs * 4)) != cudaSuccess)
+    return fail(e, JFGPU_ERR_NOMEM, "Failed to allocate the SAM/BAM batch buffers");
+  return JFGPU_OK;
+}
+
+// input bytes of the next batch: its FASTQ must fit one K1 batch and the record pool
+static size_t sam_batch_cap(const jfgpu_engine* e) {
+  return std::max<size_t>(std::min(e->sam.in_cap, part_cap_len(e, 2 * e->sam.in_cap) / 2) & ~(size_t)15, 16);
+}
+
+// Transcode the batch [dev, dev + n) that starts at byte `at` of the file (BAM: its n_recs records at the offsets in
+// sam.offs) on `st` and count the FASTQ it becomes.  *used = the input bytes transcoded (SAM: through the last newline, all
+// of them when `final`).
+static int sam_run(jfgpu_engine* e, cudaStream_t st, const uint8_t* dev, size_t n, bool final, uint32_t n_recs, uint64_t at, size_t* used) {
+  jfgpu_engine::SamState& s = e->sam;
+  const int launches = s.form == 2
+      ? jfsam::bam_transcode(dev, n, s.offs.as<uint32_t>(), n_recs, s.out.as<uint8_t>(), s.scratch.p, s.in_cap, s.res.as<jfsam::Result>(), st)
+      : jfsam::sam_transcode(dev, n, final, s.out.as<uint8_t>(), s.scratch.p, s.in_cap, s.res.as<jfsam::Result>(), st);
+  g_launches.fetch_add(launches, std::memory_order_relaxed);
+  CUDA_OK(e, cudaGetLastError());
+  CUDA_OK(e, cudaMemcpyAsync(s.h_res, s.res.p, sizeof(jfsam::Result), cudaMemcpyDeviceToHost, st));
+  CUDA_OK(e, cudaStreamSynchronize(st));
+  const jfsam::Result r = *s.h_res;
+  if(r.err) {
+    const unsigned long long v = ~r.err;
+    static const char* const what[] = { "", "fewer than 11 fields", "SEQ and QUAL of different lengths", "its fields run past its block_size" };
+    return fail(e, JFGPU_ERR_FORMAT, std::string(s.form == 2 ? "Invalid BAM record at byte " : "Invalid SAM line at byte ") +
+                std::to_string(at + (v >> 2)) + " of the " + (s.form == 2 ? "inflated " : "") + "file: " + what[v & 3]);
+  }
+  *used = s.form == 2 ? n : (size_t)r.consumed;
+  if(!r.out_bytes) return JFGPU_OK;
+  if((e->p.allow_regrow || e->spill_fn) && e->tab.slots.p) {            // as jfgpu_feed: a failed insertion regrows first
+    CUDA_OK(e, cudaMemcpyAsync(e->h_stats + STAT_FAILED, e->stats.as<unsigned long long>() + STAT_FAILED, 8, cudaMemcpyDeviceToHost, e->cs));
+    CUDA_OK(e, cudaStreamSynchronize(e->cs));
+    if(e->h_stats[STAT_FAILED]) { const int rc = check_after_batches(e); if(rc) return rc; }
+  }
+  return run_batch(e, s.out.as<uint8_t>(), r.out_bytes, r.out_bytes, st, K1_COUNT);
+}
+
+// a batch of host bytes through staging buffer 0 (free again: the previous batch was transcoded and read back)
+static int sam_stage(jfgpu_engine* e, const char* src, size_t len, bool final, uint32_t n_recs) {
+  jfgpu_engine::SamState& s = e->sam;
+  CUDA_OK(e, cudaMemcpyAsync(e->stage[0].p, src, len, cudaMemcpyHostToDevice, e->hs));
+  if(n_recs) CUDA_OK(e, cudaMemcpyAsync(s.offs.p, s.h_offs, (size_t)n_recs * 4, cudaMemcpyHostToDevice, e->hs));
+  CUDA_OK(e, cudaEventRecord(e->ev_copied[0], e->hs));
+  CUDA_OK(e, cudaStreamWaitEvent(e->cs, e->ev_copied[0], 0));
+  size_t used = 0;
+  const int rc = sam_run(e, e->cs, e->stage[0].as<uint8_t>(), len, final, n_recs, s.done_off, &used);
+  if(rc) return rc;
+  s.done_off += len;
+  return JFGPU_OK;
+}
+
+static int sam_too_long(jfgpu_engine* e) {
+  return fail(e, JFGPU_ERR_FORMAT, "a SAM line or BAM record is longer than the staging buffer (max_batch_bytes / 2)");
+}
+
+// SAM text in host memory: whole lines per batch, the incomplete last line kept for the next feed
+static int sam_feed_host(jfgpu_engine* e, const char* bytes, size_t n, bool end) {
+  jfgpu_engine::SamState& s = e->sam;
+  const size_t cap = sam_batch_cap(e);
+  size_t pos = 0;
+  int rc;
+  if(!s.tail.empty()) {                       // the line the previous feed cut, completed
+    const char* nl = n ? (const char*)memchr(bytes, '\n', n) : nullptr;
+    pos = nl ? (size_t)(nl - bytes) + 1 : n;
+    if(s.tail.size() + pos > cap) return sam_too_long(e);
+    s.tail.append(bytes, pos);
+    if(!nl && !end) return JFGPU_OK;
+    if((rc = sam_stage(e, s.tail.data(), s.tail.size(), end && pos == n, 0))) return rc;
+    s.tail.clear();
+  }
+  size_t stop = n;
+  if(!end) {
+    const char* nl = pos < n ? (const char*)memrchr(bytes + pos, '\n', n - pos) : nullptr;
+    stop = nl ? (size_t)(nl - bytes) + 1 : pos;
+  }
+  while(pos < stop) {
+    size_t len = std::min(cap, stop - pos);
+    if(pos + len < stop) {
+      const char* nl = (const char*)memrchr(bytes + pos, '\n', len);
+      if(!nl) return sam_too_long(e);
+      len = (size_t)(nl - (bytes + pos)) + 1;
+    }
+    if((rc = sam_stage(e, bytes + pos, len, end && pos + len == n, 0))) return rc;
+    pos += len;
+  }
+  if(n - pos > cap) return sam_too_long(e);
+  s.tail.assign(bytes + pos, n - pos);
+  return JFGPU_OK;
+}
+
+static uint32_t le32(const char* p) { uint32_t v; memcpy(&v, p, 4); return v; }
+
+// BAM header (SAM specification 4.2): magic and l_text, then the text; n_ref; for every reference l_name, then the name and
+// l_ref.  The text and the names are passed over.
+static int bam_header_field(jfgpu_engine* e, const char* p) {
+  jfgpu_engine::SamState& s = e->sam;
+  if(s.bam_phase == BAM_MAGIC) {
+    if(memcmp(p, "BAM\1", 4) != 0) return fail(e, JFGPU_ERR_FORMAT, "Invalid BAM magic");
+    s.bam_skip = le32(p + 4); s.bam_phase = BAM_NREF;
+  } else if(s.bam_phase == BAM_NREF) {
+    const int32_t nr = (int32_t)le32(p);
+    if(nr < 0) return fail(e, JFGPU_ERR_FORMAT, "Invalid BAM header: negative number of references");
+    s.bam_refs = (uint32_t)nr; s.bam_phase = nr ? BAM_REF : BAM_RECORDS;
+  } else {
+    s.bam_skip = (uint64_t)le32(p) + 4;
+    if(--s.bam_refs == 0) s.bam_phase = BAM_RECORDS;
+  }
+  return JFGPU_OK;
+}
+
+// bytes of a record whose block_size field is at p
+static int bam_record_len(jfgpu_engine* e, const char* p, size_t cap, size_t* len) {
+  *len = 4 + (size_t)le32(p);
+  if(*len < 36) return fail(e, JFGPU_ERR_FORMAT, "Invalid BAM record: block_size " + std::to_string(*len - 4) + " is below the 32 bytes of its fixed fields");
+  return *len > cap ? sam_too_long(e) : JFGPU_OK;
+}
+
+// The inflated BAM stream in host memory: the host walks the header and the block_size chain; the records go to the device in
+// batches with their offsets.  A header field or record the feed cuts is kept for the next feed.
+static int bam_feed_host(jfgpu_engine* e, const char* bytes, size_t n, bool end) {
+  jfgpu_engine::SamState& s = e->sam;
+  const size_t cap = sam_batch_cap(e);
+  size_t pos = 0;
+  int rc;
+  while(true) {
+    if(s.bam_skip) {
+      const size_t t = (size_t)std::min<uint64_t>(s.bam_skip, n - pos);
+      s.bam_skip -= t; pos += t; s.done_off += t;
+      if(s.bam_skip) break;
+      continue;
+    }
+    const size_t head = s.bam_phase == BAM_MAGIC ? 8 : 4;     // the bytes that give a piece's length
+    if(!s.tail.empty()) {                     // a piece the previous feed cut
+      size_t t = std::min(n - pos, head > s.tail.size() ? head - s.tail.size() : 0);
+      s.tail.append(bytes + pos, t); pos += t;
+      if(s.tail.size() < head) break;
+      size_t len = head;
+      if(s.bam_phase == BAM_RECORDS && (rc = bam_record_len(e, s.tail.data(), cap, &len))) return rc;
+      t = std::min(n - pos, len - s.tail.size());
+      s.tail.append(bytes + pos, t); pos += t;
+      if(s.tail.size() < len) break;
+      if(s.bam_phase == BAM_RECORDS) { s.h_offs[0] = 0; rc = sam_stage(e, s.tail.data(), len, false, 1); }
+      else { rc = bam_header_field(e, s.tail.data()); s.done_off += len; }
+      if(rc) return rc;
+      s.tail.clear();
+      continue;
+    }
+    if(pos == n) break;
+    if(s.bam_phase != BAM_RECORDS) {
+      if(n - pos < head) { s.tail.assign(bytes + pos, n - pos); pos = n; break; }
+      if((rc = bam_header_field(e, bytes + pos))) return rc;
+      pos += head; s.done_off += head;
+      continue;
+    }
+    // whole records in place, at most `cap` bytes per batch
+    size_t run = pos;
+    uint32_t nr = 0;
+    while(n - pos >= 4) {
+      size_t len = 0;
+      if((rc = bam_record_len(e, bytes + pos, cap, &len))) return rc;
+      if(n - pos < len) break;
+      if(pos + len - run > cap) {
+        if((rc = sam_stage(e, bytes + run, pos - run, false, nr))) return rc;
+        run = pos; nr = 0;
+      }
+      s.h_offs[nr++] = (uint32_t)(pos - run);
+      pos += len;
+    }
+    if(nr && (rc = sam_stage(e, bytes + run, pos - run, false, nr))) return rc;
+    s.tail.assign(bytes + pos, n - pos);
+    break;
+  }
+  if(end && (s.bam_phase != BAM_RECORDS || s.bam_skip || !s.tail.empty()))
+    return fail(e, JFGPU_ERR_FORMAT, s.bam_phase != BAM_RECORDS ? "Truncated BAM header" : "Truncated BAM record");
+  return JFGPU_OK;
+}
+
+// SAM text in device memory: the kernels find the last newline of every batch; the incomplete last line of the feed is kept
+// in sam.tail_dev and completed from the front of the next one
+static int sam_feed_device(jfgpu_engine* e, const uint8_t* dev, size_t n, bool end, cudaStream_t st) {
+  jfgpu_engine::SamState& s = e->sam;
+  const size_t cap = sam_batch_cap(e);
+  size_t pos = 0, used = 0;
+  int rc;
+  if(s.tail_dev_len) {
+    const size_t take = s.tail_dev_len < cap ? std::min(n, cap - s.tail_dev_len) : 0;
+    if(take < n && !take) return sam_too_long(e);
+    CUDA_OK(e, cudaMemcpyAsync(s.tail_dev.as<uint8_t>() + s.tail_dev_len, dev, take, cudaMemcpyDeviceToDevice, st));
+    const bool fin = end && take == n;
+    if((rc = sam_run(e, st, s.tail_dev.as<uint8_t>(), s.tail_dev_len + take, fin, 0, s.done_off, &used))) return rc;
+    if(!used) {                               // no newline yet
+      if(take < n) return sam_too_long(e);
+      s.tail_dev_len += take;
+      return JFGPU_OK;
+    }
+    pos = used - s.tail_dev_len; s.done_off += used; s.tail_dev_len = 0;
+  }
+  while(pos < n) {
+    const size_t len = std::min(cap, n - pos);
+    if((rc = sam_run(e, st, dev + pos, len, end && pos + len == n, 0, s.done_off, &used))) return rc;
+    if(!used) {
+      if(pos + len < n) return sam_too_long(e);
+      break;
+    }
+    pos += used; s.done_off += used;
+  }
+  if(pos < n) {
+    CUDA_OK(e, cudaMemcpyAsync(s.tail_dev.p, dev + pos, n - pos, cudaMemcpyDeviceToDevice, st));
+    s.tail_dev_len = n - pos;
+  }
+  return JFGPU_OK;
+}
+
+// jfgpu_feed / jfgpu_feed_device of a SAM or BAM file
+static int sam_feed(jfgpu_engine* e, const void* data, size_t n, uint32_t flags, bool device, cudaStream_t st) {
+  const uint32_t form = flags & JFGPU_FORMAT_BAM ? 2 : flags & JFGPU_FORMAT_SAM ? 1 : 0;
+  if((flags & SAM_FLAGS) == SAM_FLAGS) return fail(e, JFGPU_ERR_ARG, "JFGPU_FORMAT_SAM and JFGPU_FORMAT_BAM exclude each other");
+  if(!(flags & JFGPU_FILE_BEGIN) && form && form != e->sam.form) return fail(e, JFGPU_ERR_ARG, "the format flag differs from the one the file began with");
+  if(device && (flags & JFGPU_FILE_BEGIN ? form : e->sam.form) == 2) return fail(e, JFGPU_ERR_ARG, "BAM input is taken from host memory only (jfgpu_feed)");
+  int rc = begin_feed(e, flags, -1, st);
+  if(rc) return rc;
+  if((rc = sam_alloc(e))) return rc;
+  if(e->part.P) { rc = part_alloc(e); if(rc) return rc; }
+  const bool end = flags & JFGPU_FILE_END;
+  cudaEventRecord(e->ev_t0, st);
+  if(device) rc = sam_feed_device(e, (const uint8_t*)data, n, end, st);
+  else if(e->sam.form == 2) rc = bam_feed_host(e, (const char*)data, n, end);
+  else rc = sam_feed_host(e, (const char*)data, n, end);
+  if(rc) return rc;
+  cudaEventRecord(e->ev_t1, st);
+  CUDA_OK(e, cudaStreamSynchronize(st));
+  { float ms = 0; cudaEventElapsedTime(&ms, e->ev_t0, e->ev_t1); e->count_ms += ms; }
+  resolve_kernel_events(e);
+  e->bytes_fed += n;
+  if(e->tab.slots.p) { rc = check_after_batches(e); if(rc) return rc; }
+  return end_feed(e, flags, st);
+}
+
 int jfgpu_feed_device(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_t flags, void* stream) {
   if(!e) return JFGPU_ERR_ARG;
   if(((uintptr_t)dev_bytes & 15) != 0) return fail(e, JFGPU_ERR_ARG, "device text must be 16-byte aligned");
   cudaSetDevice(e->device);
   cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
+  if((flags & SAM_FLAGS) || (e->sam.form && !(flags & JFGPU_FILE_BEGIN))) return sam_feed(e, dev_bytes, n, flags, true, st);
   int rc = begin_device_feed(e, flags, dev_bytes, n, st);
   if(rc) return rc;
   const uint8_t* p = (const uint8_t*)dev_bytes;
@@ -1643,6 +1917,7 @@ static int next_batch_len(jfgpu_engine* e, const char* bytes, size_t off, size_t
 int jfgpu_feed(jfgpu_handle e, const char* bytes, size_t n, uint32_t flags) {
   if(!e) return JFGPU_ERR_ARG;
   cudaSetDevice(e->device);
+  if((flags & SAM_FLAGS) || (e->sam.form && !(flags & JFGPU_FILE_BEGIN))) return sam_feed(e, bytes, n, flags, false, e->cs);
   int rc = begin_feed(e, flags, n ? (unsigned char)bytes[0] : (e->q_tail.empty() ? -1 : (unsigned char)e->q_tail[0]), e->cs);
   if(rc) return rc;
   if(flags & JFGPU_FILE_BEGIN) { e->q_lines = 0; e->q_tail.clear(); }
@@ -1692,6 +1967,7 @@ int jfgpu_feed(jfgpu_handle e, const char* bytes, size_t n, uint32_t flags) {
 int jfgpu_extract_route(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_t flags, void* dev_keys, uint64_t capacity,
                         uint64_t* dev_counts, void* stream) {
   if(!e) return JFGPU_ERR_ARG;
+  if(flags & SAM_FLAGS) return fail(e, JFGPU_ERR_ARG, "jfgpu_extract_route takes no SAM or BAM input");
   if(!e->tab.slots.p) return fail(e, JFGPU_ERR_STATE, "this engine holds a Bloom counter, not a hash table");
   if(((uintptr_t)dev_bytes & 15) != 0) return fail(e, JFGPU_ERR_ARG, "device text must be 16-byte aligned");
   if(e->kw == 4 && ((uintptr_t)dev_keys & 15) != 0) return fail(e, JFGPU_ERR_ARG, "route buckets of four-word keys must be 16-byte aligned");
@@ -1766,6 +2042,7 @@ uint64_t jfgpu_shard_round_bytes(jfgpu_handle e) {
 
 int jfgpu_shard_extract(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_t flags, uint32_t bank, void* stream) {
   if(!e) return JFGPU_ERR_ARG;
+  if(flags & SAM_FLAGS) return fail(e, JFGPU_ERR_ARG, "the record exchange takes no SAM or BAM input");
   if(!e->sh.on || bank > 1) return fail(e, JFGPU_ERR_STATE, "jfgpu_shard_setup has not been called");
   // the record exchange's send kernels apply no Bloom structure: one attached after jfgpu_shard_setup would be ignored
   if(e->bloom.mode != BLOOM_NONE) return fail(e, JFGPU_ERR_STATE, "the record exchange takes no Bloom filter (use the key exchange)");
@@ -2285,6 +2562,7 @@ static int query_impl(jfgpu_engine* e, const char* bytes, size_t n, uint32_t fla
 
 int jfgpu_query(jfgpu_handle e, const char* bytes, size_t n, uint32_t flags, jfgpu_sink_fn sink, void* ctx, uint64_t* n_kmers) {
   if(!e || !sink || (n && !bytes)) return JFGPU_ERR_ARG;
+  if(flags & SAM_FLAGS) return fail(e, JFGPU_ERR_ARG, "a query takes no SAM or BAM input");
   if(n_kmers) *n_kmers = 0;
   if(!e->tab.slots.p) return fail(e, JFGPU_ERR_STATE, "this engine holds a Bloom counter, not a hash table");
   if(e->shard_bits) return fail(e, JFGPU_ERR_STATE, "a query needs the whole table, not a shard");

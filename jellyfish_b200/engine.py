@@ -129,9 +129,9 @@ class HashCounter(object):
             ptr, n = C.cast(C.c_char_p(buf), C.c_void_p), len(buf)
         self._check(self._lib.jfgpu_feed(self._h, ptr, n, flags))
 
-    def add_device_text(self, dev_ptr, n, begin=True, end=True, stream=None):
-        """Same with the text already in device memory (e.g. a torch uint8 tensor's data_ptr())."""
-        flags = (L.FILE_BEGIN if begin else 0) | (L.FILE_END if end else 0)
+    def add_device_text(self, dev_ptr, n, begin=True, end=True, stream=None, sam=False):
+        """Same with the text already in device memory (e.g. a torch uint8 tensor's data_ptr()); sam=True: SAM text."""
+        flags = (L.FILE_BEGIN if begin else 0) | (L.FILE_END if end else 0) | (L.FORMAT_SAM if sam else 0)
         self._check(self._lib.jfgpu_feed_device(self._h, C.c_void_p(dev_ptr), n, flags, C.c_void_p(stream or 0)))
 
     def add_files(self, paths, chunk=64 << 20):
@@ -145,6 +145,40 @@ class HashCounter(object):
                 while True:
                     nxt = f.read(chunk)
                     self.add_text(cur, begin=first, end=not nxt)
+                    first = False
+                    if not nxt:
+                        break
+                    cur = nxt
+
+    def add_sam_text(self, data, begin=True, end=True, bam=False):
+        """Count the reads of SAM text, or (bam=True) of an inflated BAM stream, held in host memory (bytes or a pointer/size
+        pair): each record's SEQ with its QUAL, as `count --sam` does (include/jfgpu.h: JFGPU_FORMAT_SAM / _BAM).  A file
+        may come in any number of pieces, cut anywhere; `begin` and `end` mark its first and last."""
+        flags = (L.FILE_BEGIN if begin else 0) | (L.FILE_END if end else 0) | (L.FORMAT_BAM if bam else L.FORMAT_SAM)
+        if isinstance(data, tuple):
+            ptr, n = data
+        else:
+            buf = bytes(data)
+            ptr, n = C.cast(C.c_char_p(buf), C.c_void_p), len(buf)
+        self._check(self._lib.jfgpu_feed(self._h, ptr, n, flags))
+
+    def add_sam_files(self, paths, chunk=64 << 20):
+        """`count --sam` over a list of files: SAM text, gzip'd SAM or BAM, told apart by their magic.  CRAM is refused."""
+        import gzip
+        for path in paths:
+            with open(path, "rb") as raw:
+                magic = raw.read(4)
+            if magic.startswith(b"CRAM"):
+                raise JellyfishError(L.ERR_FORMAT, "CRAM input is not supported ('%s')" % path)
+            # (BGZF is multi-member gzip: the gzip module reads it whole)
+            f = gzip.open(path, "rb") if magic[:2] == b"\x1f\x8b" else open(path, "rb")
+            with f:
+                cur = f.read(chunk)
+                bam = cur[:4] == b"BAM\1"
+                first = True
+                while True:
+                    nxt = f.read(chunk) if cur else b""
+                    self.add_sam_text(cur, begin=first, end=not nxt, bam=bam)
                     first = False
                     if not nxt:
                         break
