@@ -51,7 +51,14 @@ enum {
    * fields, SEQ and QUAL of different lengths, a BAM record or header cut short or with a bad magic) fails the feed with
    * JFGPU_ERR_FORMAT.  jfgpu_query, jfgpu_extract_route and jfgpu_shard_extract take neither flag (JFGPU_ERR_ARG). */
   JFGPU_FORMAT_SAM = 4u,
-  JFGPU_FORMAT_BAM = 8u
+  JFGPU_FORMAT_BAM = 8u,
+  /* Text that starts in the middle of a file (a share of one file split among ranks).  Given with JFGPU_FILE_BEGIN, the bytes
+   * start at a line start of a file of this format and the first byte is not sniffed.  FASTA: the parser starts at a line
+   * start (a share may begin on a sequence line).  FASTQ: the parser starts with a record's header line expected.  Taken by
+   * jfgpu_feed, jfgpu_feed_device, jfgpu_extract_route, jfgpu_shard_extract, jfgpu_query and jfgpu_seam; the two exclude each
+   * other and the SAM / BAM flags. */
+  JFGPU_FORMAT_FASTA = 16u,
+  JFGPU_FORMAT_FASTQ = 32u
 };
 
 /* operations of mer_counter_base (sub_commands/count_main.cc:133,152-184) */
@@ -172,6 +179,22 @@ int  jfgpu_feed(jfgpu_handle h, const char* bytes, size_t n, uint32_t flags);
 /* Same with the text already resident in device memory (16-byte aligned pointer).
  * `stream` is a cudaStream_t (NULL = the engine's own stream). */
 int  jfgpu_feed_device(jfgpu_handle h, const void* dev_bytes, size_t n, uint32_t flags, void* stream);
+
+/* -- the seam in front of a share of a file (no reference analogue: the reference reads every file whole).  Parse the text
+ *    [dev_bytes, dev_bytes + n) and keep only what a feed leaves to the next one: the parser state and the last symbols
+ *    (the k-1 base seam).  Nothing is counted: no table, route bucket or Bloom structure is touched and the statistics do not
+ *    change.  The next call of jfgpu_feed, jfgpu_feed_device, jfgpu_extract_route or jfgpu_shard_extract without
+ *    JFGPU_FILE_BEGIN continues from there, so that a seam of the text in front of a share followed by the share counts the
+ *    k-mers of the share exactly as a feed of the whole file would.  Flags as for a feed (JFGPU_FILE_BEGIN with
+ *    JFGPU_FORMAT_FASTA / _FASTQ in front of a share; JFGPU_FILE_END is refused, SAM and BAM too).  An engine with min_qual
+ *    (-Q) is refused (JFGPU_ERR_ARG): its parser has other '\r' rules.  Synchronises `stream` (NULL = the engine's own).
+ *    jfgpu_seam_host takes the text from HOST memory, as jfgpu_feed does. */
+int  jfgpu_seam(jfgpu_handle h, const void* dev_bytes, size_t n, uint32_t flags, void* stream);
+int  jfgpu_seam_host(jfgpu_handle h, const char* bytes, size_t n, uint32_t flags);
+/* Add the number of '\n' bytes of [dev_bytes, dev_bytes + n) (device memory, any alignment) to *dev_count (a device uint64
+ * the caller zeroes).  Stream-ordered on `stream` (NULL = the engine's own stream); the caller synchronises before reading
+ * the count.  Used to check that the shares of a FASTQ file start on record boundaries. */
+int  jfgpu_count_newlines(jfgpu_handle h, const void* dev_bytes, size_t n, uint64_t* dev_count, void* stream);
 
 /* -- multi-GPU stages (no reference analogue; SURVEY.md section 8e) ------------------
  * Extract canonical k-mers from device-resident text and bucket them by owning shard

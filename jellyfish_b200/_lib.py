@@ -19,12 +19,13 @@ SYMBOLS = [
     "jfgpu_host_alloc", "jfgpu_host_free", "jfgpu_memcpy_h2d", "jfgpu_kernel_launches", "jfgpu_version",
     "jfgpu_bloom_info_get", "jfgpu_bloom_load", "jfgpu_bloom_dump", "jfgpu_bloom_words", "jfgpu_bloom_fold", "jfgpu_bloom_dump_range",
     "jfgpu_set_spill", "jfgpu_shard_setup", "jfgpu_shard_round_bytes", "jfgpu_shard_extract", "jfgpu_shard_pack", "jfgpu_shard_unpack",
-    "jfgpu_load_records", "jfgpu_query", "jfgpu_device_count",
+    "jfgpu_load_records", "jfgpu_query", "jfgpu_device_count", "jfgpu_seam", "jfgpu_seam_host", "jfgpu_count_newlines",
 ]
 
 OK, ERR_ARG, ERR_CUDA, ERR_FULL, ERR_FORMAT, ERR_STATE, ERR_NOMEM, ERR_SINK = range(8)
 FILE_BEGIN, FILE_END = 1, 2
 FORMAT_SAM, FORMAT_BAM = 4, 8
+FORMAT_FASTA, FORMAT_FASTQ = 16, 32
 
 
 class Params(C.Structure):
@@ -162,6 +163,12 @@ def load():
     lib.jfgpu_load_records.restype = C.c_int
     lib.jfgpu_query.argtypes = [H, C.c_void_p, C.c_size_t, C.c_uint32, SINK_FN, C.c_void_p, C.POINTER(C.c_uint64)]
     lib.jfgpu_query.restype = C.c_int
+    lib.jfgpu_seam.argtypes = [H, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p]
+    lib.jfgpu_seam.restype = C.c_int
+    lib.jfgpu_seam_host.argtypes = [H, C.c_void_p, C.c_size_t, C.c_uint32]
+    lib.jfgpu_seam_host.restype = C.c_int
+    lib.jfgpu_count_newlines.argtypes = [H, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    lib.jfgpu_count_newlines.restype = C.c_int
     lib.jfgpu_device_count.argtypes = []
     lib.jfgpu_device_count.restype = C.c_int
     _lib = lib

@@ -3,8 +3,19 @@
     torchrun --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 -m jellyfish_b200.count_multi \
         -m 21 -s 16G -C -o mer_counts.jf reads_1.fa reads_2.fa ...
 
-Every rank parses the files `files[rank::N]` (a file is the unit of distribution: no k-mer spans two
-files, mer_overlap_sequence_parser.hpp:111), the k-mers are routed to the rank that owns their table
+With `--split auto` (the default) every file is split among the ranks (jellyfish_b200/split.py): rank r counts the bytes
+from the first line start at or after r/N of the file -- for FASTQ the first line where two records look whole -- up to
+where rank r+1's share starts.  A FASTA share that starts in the middle of a sequence first parses a seam of whole lines in
+front of it without counting them (jfgpu_seam), so the k-mers that span the cut are counted once, by the rank the cut
+starts.  Each rank reads its share with pread into two pinned buffers of one exchange round each, so a file may be larger
+than host or device memory.  The FASTQ cuts are checked after the count: every rank tallies the newlines of its share on
+the device and the tallies are gathered; if a share does not start behind a multiple of 4 lines (a sequence line that
+starts with '@' and a quality line that starts with '+' can fool the local rule), every rank clears its table and the
+files are counted again with `--split files`, with a note on stderr.  A path that is not a regular file (a pipe, a
+process substitution such as `<(zcat reads.fq.gz)`) cannot be read at offsets: it is counted whole by one rank, as with
+`--split files`.  `--split files`: every rank parses the files
+`files[rank::N]` whole (a file is the unit of distribution: no k-mer spans two
+files, mer_overlap_sequence_parser.hpp:111).  Either way the k-mers are routed to the rank that owns their table
 position, each rank writes `OUT.<rank>`, and rank 0 concatenates the shards in rank order into OUT --
 byte-identical to what one GPU (or the reference) writes for the same input, since shard r holds
 exactly the positions r*size/N ... (r+1)*size/N - 1.  (`jellyfish merge` on the shard files gives the
@@ -22,12 +33,72 @@ import sys
 import torch
 import torch.distributed as dist
 
-from .distributed import ShardedCounter, concat_shards
+from .distributed import ShardedCounter, ShareReader, concat_shards, fastq_cuts_agree
+from .split import plan_file, splittable
 
 
 def _size(v):
     mult = {"k": 10**3, "M": 10**6, "G": 10**9, "T": 10**12}
     return int(v[:-1]) * mult[v[-1]] if v[-1] in mult else int(v)
+
+
+def _count_whole(sc, path, owner):
+    """One file read whole by one rank and counted from device memory; every other rank takes part in the exchange rounds."""
+    if not owner:
+        sc.add_device_text(0, 0)
+        return
+    with open(path, "rb") as f:
+        data = f.read()
+    if data[:1] not in (b">", b"@", b""):
+        raise SystemExit("Unsupported format: %s" % path)
+    buf = torch.zeros(max(16, len(data) + 256), dtype=torch.uint8, device="cuda")
+    if data:
+        buf[:len(data)] = torch.frombuffer(bytearray(data), dtype=torch.uint8).cuda()
+    sc.add_device_text(buf.data_ptr(), len(data))
+
+
+def count_files(sc, files, rank, world):
+    """--split files: rank r counts files[r::world], each whole and resident in device memory."""
+    mine = files[rank::world]
+    rounds = torch.tensor([len(mine)], device="cuda")
+    if world > 1:
+        dist.all_reduce(rounds, op=dist.ReduceOp.MAX)       # every rank takes part in every exchange
+    for i in range(int(rounds.item())):
+        if i < len(mine):
+            _count_whole(sc, mine[i], True)
+        else:
+            sc.add_device_text(0, 0)
+
+
+def count_split(sc, files, rank, world, k):
+    """--split auto: every regular file split among the ranks and streamed (see the module documentation); anything else
+    (a pipe, a process substitution) counted whole by rank i % world, as --split files would.  Returns False when a FASTQ
+    share did not start on a record: the table then holds a wrong count and must be cleared."""
+    tallies = []
+    for i, path in enumerate(files):
+        if not splittable(path):
+            _count_whole(sc, path, i % world == rank)
+            continue
+        try:
+            share = plan_file(path, rank, world, k)
+        except ValueError:
+            raise SystemExit("Unsupported format: %s" % path)
+        if share is None:                      # an empty file holds no k-mer
+            continue
+        reader = ShareReader(path, share, sc.piece_bytes())
+        try:
+            seam = reader.seam()
+            if seam:
+                t = torch.frombuffer(bytearray(seam), dtype=torch.uint8).cuda()
+                sc.hc.seam(t.data_ptr(), len(seam), fmt=share.fmt)
+                del t
+            tally = torch.zeros(1, dtype=torch.int64, device="cuda") if share.fmt == "fastq" else None
+            sc.add_pieces(reader, tally)
+        finally:
+            reader.close()
+        if tally is not None:
+            tallies.append([share.end - share.start, int(tally.item())])
+    return fastq_cuts_agree(tallies, world, "cuda")
 
 
 def main(argv=None):
@@ -45,6 +116,8 @@ def main(argv=None):
     ap.add_argument("--bf-fp", type=float, default=0.01, help="false positive rate of the Bloom prefilter")
     ap.add_argument("--bc", help="count only the k-mers this Bloom counter (written by `bc`) holds twice")
     ap.add_argument("--keep-shards", action="store_true")
+    ap.add_argument("--split", choices=("auto", "files"), default="auto",
+                    help="auto: split every file among the ranks; files: give rank r the whole files files[r::N]")
     ap.add_argument("files", nargs="+")
     a = ap.parse_args(argv)
     # the single-GPU command's checks (count_main.cc:196-197 and the k <= 64 scope of every Bloom structure)
@@ -64,23 +137,13 @@ def main(argv=None):
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     sc = ShardedCounter(a.size, a.counter_len, k=a.mer_len, canonical=a.canonical, rank=rank, world=world, device=local,
                         reprobes=a.reprobes, bf_size=a.bf_size, bf_fp=a.bf_fp, bc=a.bc)
-    mine = a.files[rank::world]
-    rounds = torch.tensor([len(mine)], device="cuda")
-    if world > 1:
-        dist.all_reduce(rounds, op=dist.ReduceOp.MAX)       # every rank takes part in every exchange
-    for i in range(int(rounds.item())):
-        if i < len(mine):
-            with open(mine[i], "rb") as f:
-                data = f.read()
-            if data[:1] not in (b">", b"@", b""):
-                raise SystemExit("Unsupported format: %s" % mine[i])
-            buf = torch.zeros(max(16, len(data) + 256), dtype=torch.uint8, device="cuda")
-            if data:
-                buf[:len(data)] = torch.frombuffer(bytearray(data), dtype=torch.uint8).cuda()
-            sc.add_device_text(buf.data_ptr(), len(data))
-            del buf
-        else:
-            sc.add_device_text(0, 0)
+    if a.split == "files":
+        count_files(sc, a.files, rank, world)
+    elif not count_split(sc, a.files, rank, world, a.mer_len):
+        if rank == 0:
+            sys.stderr.write("count_multi: a FASTQ share does not start on a record; counting whole files per rank instead\n")
+        sc.hc.clear()
+        count_files(sc, a.files, rank, world)
     st = sc.done()
     cmdline = ["count_multi"] + (argv if argv is not None else sys.argv[1:])
     sc.hc.dump("%s.%d" % (a.output, rank), lower=a.lower_count, upper=a.upper_count, out_counter_len=a.out_counter_len, cmdline=cmdline)

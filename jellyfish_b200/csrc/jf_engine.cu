@@ -23,6 +23,7 @@
 #include "jf_wide.cuh"
 #include "jf_bloom.cuh"
 #include "jf_sam.cuh"
+#include "jf_newline.cuh"
 
 using namespace jfk;
 
@@ -35,6 +36,7 @@ namespace {
 
 constexpr unsigned SHARD_RESERVED_SMS = 16;
 constexpr uint32_t SAM_FLAGS = JFGPU_FORMAT_SAM | JFGPU_FORMAT_BAM;
+constexpr uint32_t TEXT_FLAGS = JFGPU_FORMAT_FASTA | JFGPU_FORMAT_FASTQ;
 constexpr uint64_t WIN_DEF_CAP = (uint64_t)16 << 20;   // deferred records per group of the window form of K2   // SMs K1 leaves to NCCL while an exchange runs beside it
 
 unsigned ceil_log2(uint64_t x) { unsigned l = 0; while(l < 64 && ((uint64_t)1 << l) < x) ++l; return l; }
@@ -231,6 +233,9 @@ struct jfgpu_engine {
   } qb[2];
   HostBuf<uint8_t> q_host[2]; Event ev_qcopy[2];
   uint64_t q_tiles_cap = 0; int q_cur = 0;
+  // jfgpu_seam: the ordered extraction runs into scratch that nobody reads (only the carry it leaves matters)
+  bool seaming = false;
+  DevBuf seam_keys, seam_cnt;
   // SAM / BAM input (jf_sam.cu): the form of the file being fed (0 = FASTA / FASTQ text, 1 = SAM, 2 = BAM), the buffers of a
   // batch (made at the first such file; one of each: a batch is transcoded and read back before the next is staged) and what
   // a feed leaves to the next one
@@ -1013,7 +1018,8 @@ int run_batch(jfgpu_engine* e, const uint8_t* dev, uint64_t n, uint64_t n_look, 
   a.route_keys = route_keys; a.route_counts = route_counts; a.route_cap = route_cap; a.shard_bits = e->shard_bits;
   if(query) {                                   // no hash, no filter: the keys themselves, in input order
     a.lut = nullptr; a.lut_bytes = 0; a.hash_fast = 0; memset(&a.bloom, 0, sizeof(a.bloom));
-    a.q_keys = e->qb[e->q_cur].keys.as<uint64_t>(); a.q_cnt = e->qb[e->q_cur].cnt.as<uint32_t>(); a.q_tile_cap = tile;
+    a.q_keys = (e->seaming ? e->seam_keys : e->qb[e->q_cur].keys).as<uint64_t>();
+    a.q_cnt = (e->seaming ? e->seam_cnt : e->qb[e->q_cur].cnt).as<uint32_t>(); a.q_tile_cap = tile;
   }
   PartDev pd = shard_send ? shard_send_dev(e, bank) : part_dev(e);
   auto launch = [&](auto kern, int nth, size_t smem, bool one_per_sm) -> int {
@@ -1532,12 +1538,15 @@ void jfgpu_destroy(jfgpu_handle e) {
 }
 
 static int begin_feed(jfgpu_engine* e, uint32_t flags, int first_byte, cudaStream_t st) {
+  if((flags & TEXT_FLAGS) == TEXT_FLAGS || ((flags & TEXT_FLAGS) && (flags & SAM_FLAGS)))
+    return fail(e, JFGPU_ERR_ARG, "JFGPU_FORMAT_FASTA, _FASTQ, _SAM and _BAM exclude each other");
   if(flags & JFGPU_FILE_BEGIN) {
-    // mer_overlap_sequence_parser.hpp:134-148: the first byte selects the format, unless the caller gives SAM or BAM
+    // mer_overlap_sequence_parser.hpp:134-148: the first byte selects the format, unless the caller gives it (a share that
+    // starts in the middle of a file, or SAM / BAM)
     const uint32_t form = flags & JFGPU_FORMAT_BAM ? 2 : flags & JFGPU_FORMAT_SAM ? 1 : 0;
-    if(!form && first_byte >= 0 && first_byte != '>' && first_byte != '@') return fail(e, JFGPU_ERR_FORMAT, "Unsupported format");
+    if(!form && !(flags & TEXT_FLAGS) && first_byte >= 0 && first_byte != '>' && first_byte != '@') return fail(e, JFGPU_ERR_FORMAT, "Unsupported format");
     // SAM and BAM records reach the extraction kernels as 4-line FASTQ
-    e->format = form || first_byte == '@' ? 1 : 0;
+    e->format = form || (flags & JFGPU_FORMAT_FASTQ) || (!(flags & JFGPU_FORMAT_FASTA) && first_byte == '@') ? 1 : 0;
     e->sam.form = form; e->sam.tail.clear(); e->sam.tail_dev_len = 0;
     e->sam.bam_phase = 0; e->sam.bam_refs = 0; e->sam.bam_skip = 0; e->sam.done_off = 0;
     int rc = reset_carry(e, st);
@@ -1829,6 +1838,7 @@ static int sam_feed_device(jfgpu_engine* e, const uint8_t* dev, size_t n, bool e
 // jfgpu_feed / jfgpu_feed_device of a SAM or BAM file
 static int sam_feed(jfgpu_engine* e, const void* data, size_t n, uint32_t flags, bool device, cudaStream_t st) {
   const uint32_t form = flags & JFGPU_FORMAT_BAM ? 2 : flags & JFGPU_FORMAT_SAM ? 1 : 0;
+  if(flags & TEXT_FLAGS) return fail(e, JFGPU_ERR_ARG, "JFGPU_FORMAT_FASTA, _FASTQ, _SAM and _BAM exclude each other");
   if((flags & SAM_FLAGS) == SAM_FLAGS) return fail(e, JFGPU_ERR_ARG, "JFGPU_FORMAT_SAM and JFGPU_FORMAT_BAM exclude each other");
   if(!(flags & JFGPU_FILE_BEGIN) && form && form != e->sam.form) return fail(e, JFGPU_ERR_ARG, "the format flag differs from the one the file began with");
   if(device && (flags & JFGPU_FILE_BEGIN ? form : e->sam.form) == 2) return fail(e, JFGPU_ERR_ARG, "BAM input is taken from host memory only (jfgpu_feed)");
@@ -1962,6 +1972,91 @@ int jfgpu_feed(jfgpu_handle e, const char* bytes, size_t n, uint32_t flags) {
   resolve_kernel_events(e);
   if(e->tab.slots.p) { rc = check_after_batches(e); if(rc) return rc; }
   return end_feed(e, flags, e->cs);
+}
+
+// ---- jfgpu_seam: the ordered extraction of a query (K1 MODE 3) over text whose k-mers are not wanted, for the parser state
+// and the last symbols it leaves in the carry.  The k-mers go to scratch nobody reads; no table, bucket or filter is touched.
+constexpr size_t SEAM_BATCH = (size_t)1 << 20;          // text per launch (the scratch holds the k-mers of that much)
+
+static int seam_begin(jfgpu_engine* e, uint32_t flags, cudaStream_t st, unsigned long long* fmt_err0) {
+  if(e->p.min_qual) return fail(e, JFGPU_ERR_ARG, "jfgpu_seam: an engine with min_qual (-Q) reads '\\r' by other rules");
+  if(flags & (SAM_FLAGS | JFGPU_FILE_END)) return fail(e, JFGPU_ERR_ARG, "jfgpu_seam takes neither JFGPU_FILE_END nor SAM or BAM input");
+  if(e->sam.form && !(flags & JFGPU_FILE_BEGIN)) return fail(e, JFGPU_ERR_ARG, "jfgpu_seam cannot continue a SAM or BAM file");
+  if(!e->seam_keys.p) {
+    const uint64_t TILE = 512 * 32 - HALO, tiles = (SEAM_BATCH + TILE - 1) / TILE;
+    if(make_all(need(e->seam_keys, tiles * TILE * 8 * e->kw), need(e->seam_cnt, tiles * 4)) != cudaSuccess)
+      return fail(e, JFGPU_ERR_NOMEM, "allocation of the seam scratch failed");
+  }
+  CUDA_OK(e, cudaStreamSynchronize(st));
+  const int rc = read_stats(e);
+  *fmt_err0 = e->h_stats[STAT_FORMAT_ERR];
+  return rc;
+}
+
+// a FASTQ record the device parser cannot read counts as a format error of the counted text: the seam reports it itself
+static int seam_end(jfgpu_engine* e, int rc, cudaStream_t st, unsigned long long fmt_err0) {
+  e->seaming = false;
+  if(rc) return rc;
+  CUDA_OK(e, cudaStreamSynchronize(st));
+  rc = read_stats(e);
+  if(rc) return rc;
+  if(e->h_stats[STAT_FORMAT_ERR] != fmt_err0) {
+    CUDA_OK(e, cudaMemcpyAsync(e->stats.as<unsigned long long>() + STAT_FORMAT_ERR, &fmt_err0, 8, cudaMemcpyHostToDevice, e->cs));
+    CUDA_OK(e, cudaStreamSynchronize(e->cs));
+    e->h_stats[STAT_FORMAT_ERR] = fmt_err0;
+    end_feed(e, JFGPU_FILE_END, e->cs);
+    return fail(e, JFGPU_ERR_FORMAT, "Invalid fastq sequence (the device parser reads 4-line FASTQ records: '@' header, sequence, '+', qualities)");
+  }
+  return JFGPU_OK;
+}
+
+int jfgpu_seam(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_t flags, void* stream) {
+  if(!e || (n && !dev_bytes)) return JFGPU_ERR_ARG;
+  if(((uintptr_t)dev_bytes & 15) != 0) return fail(e, JFGPU_ERR_ARG, "device text must be 16-byte aligned");
+  cudaSetDevice(e->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
+  unsigned long long fmt_err0 = 0;
+  int rc = seam_begin(e, flags, st, &fmt_err0);
+  if(!rc) rc = begin_device_feed(e, flags, dev_bytes, n, st);
+  if(rc) return rc;
+  e->seaming = true;
+  const uint8_t* p = (const uint8_t*)dev_bytes;
+  for(size_t off = 0; off < n && !rc; ) {
+    const size_t len = std::min(SEAM_BATCH, n - off);
+    rc = run_batch(e, p + off, len, n - off, st, K1_QUERY, off);
+    off += len;
+  }
+  return seam_end(e, rc, st, fmt_err0);
+}
+
+int jfgpu_seam_host(jfgpu_handle e, const char* bytes, size_t n, uint32_t flags) {
+  if(!e || (n && !bytes)) return JFGPU_ERR_ARG;
+  cudaSetDevice(e->device);
+  unsigned long long fmt_err0 = 0;
+  int rc = seam_begin(e, flags, e->cs, &fmt_err0);
+  if(!rc) rc = begin_feed(e, flags, n ? (unsigned char)bytes[0] : -1, e->cs);
+  if(rc) return rc;
+  for(int i = 0; i < 2; ++i) if(!e->stage[i].p) CUDA_OK(e, e->stage[i].alloc(e->batch_bytes + 64));
+  e->seaming = true;
+  for(size_t off = 0; off < n && !rc; ) {
+    size_t len = 0;
+    rc = next_batch_len(e, bytes, off, n, std::min(std::min(SEAM_BATCH, e->batch_bytes), n - off), false, &len);
+    if(rc) break;
+    // the previous batch that used this staging buffer must be done before it is overwritten
+    CUDA_OK(e, cudaEventSynchronize(e->ev_done[e->stage_cur]));
+    rc = run_staged(e, bytes, off, len, n, K1_QUERY);
+    off += len;
+  }
+  return seam_end(e, rc, e->cs, fmt_err0);
+}
+
+int jfgpu_count_newlines(jfgpu_handle e, const void* dev_bytes, size_t n, uint64_t* dev_count, void* stream) {
+  if(!e || (n && (!dev_bytes || !dev_count))) return JFGPU_ERR_ARG;
+  cudaSetDevice(e->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
+  g_launches.fetch_add(jfnl::count_newlines((const uint8_t*)dev_bytes, n, (unsigned long long*)dev_count, e->n_sm, st), std::memory_order_relaxed);
+  CUDA_OK(e, cudaGetLastError());
+  return JFGPU_OK;
 }
 
 int jfgpu_extract_route(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_t flags, void* dev_keys, uint64_t capacity,

@@ -140,42 +140,69 @@ class RecordExchange(object):
     def add_device_text(self, ptr, n, begin, end):
         self._rounds(n, begin, end, lambda off, ln, bank: ptr + off)
 
-    def add_host_text(self, hptr, n, begin, end):
-        """Pinned host text: every round's slice is copied to a device staging buffer (one per bank) on the extraction stream."""
+    def _staged(self, hptr, ln, bank):
+        """Copy ln bytes of pinned host text into the device staging buffer of `bank` on the extraction stream."""
         import ctypes as C
         from . import _lib
-        lib = _lib.load()
         if getattr(self, "_stage", None) is None:
             self._stage = [torch.empty(self.round_bytes + 256, dtype=torch.uint8, device=self.dev) for _ in range(2)]
+        dst = self._stage[bank].data_ptr()
+        if ln and _lib.load().jfgpu_memcpy_h2d(C.c_void_p(dst), C.c_void_p(hptr), ln, C.c_void_p(self.sa.cuda_stream)):
+            raise RuntimeError("host to device copy failed")
+        return dst
 
-        def fetch(off, ln, bank):
-            dst = self._stage[bank].data_ptr()
-            if ln and lib.jfgpu_memcpy_h2d(C.c_void_p(dst), C.c_void_p(hptr + off), ln, C.c_void_p(self.sa.cuda_stream)):
-                raise RuntimeError("host to device copy failed")
-            return dst
-        self._rounds(n, begin, end, fetch)
+    def add_host_text(self, hptr, n, begin, end):
+        """Pinned host text: every round's slice is copied to a device staging buffer (one per bank) on the extraction stream."""
+        self._rounds(n, begin, end, lambda off, ln, bank: self._staged(hptr + off, ln, bank))
+
+    def add_pieces(self, reader, tally=None):
+        """A share of a file, piece by piece (ShareReader): piece i is read into pinned memory, copied to the staging buffer
+        of its bank and extracted while the exchange of piece i - 1 runs.  tally: a device int64 the newlines of every piece
+        are added to."""
+        def extract(r, bank):
+            if r >= reader.n_pieces:
+                return
+            hptr, ln, begin, end = reader.read(r)
+            src = self._staged(hptr, ln, bank)
+            reader.release(r, self.sa)
+            reader.prefetch(r + 1)
+            if tally is not None:
+                self.hc.count_newlines(src, ln, tally.data_ptr(), stream=self.sa.cuda_stream)
+            self.hc.shard_extract(src, ln, bank, begin, end, stream=self.sa.cuda_stream, fmt=reader.fmt)
+        self._run(reader.n_pieces, extract)
 
     def _rounds(self, n, begin, end, fetch):
-        w = self.world
         rounds = (n + self.round_bytes - 1) // self.round_bytes if n else 0
+
+        def extract(r, bank):
+            off = r * self.round_bytes
+            ln = max(0, min(self.round_bytes, n - off))
+            if ln or (r == 0 and begin) or (r == rounds_all[0] - 1 and end):
+                src = fetch(off, ln, bank)
+                self.hc.shard_extract(src, ln, bank, begin and r == 0, end and off + ln >= n, stream=self.sa.cuda_stream)
+        rounds_all = [0]
+        self._run(rounds, extract, rounds_all)
+
+    def _run(self, rounds, extract, rounds_out=None):
+        """Every rank takes part in max(rounds over the ranks, 1) exchange rounds; extract(r, bank) files round r's records
+        into send bank `bank` on the extraction stream (nothing when this rank has no text for the round)."""
+        w = self.world
         t = torch.tensor([rounds], dtype=torch.int64, device=self.dev)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         rounds_all = max(int(t.item()), 1)        # every rank takes part in every exchange
+        if rounds_out is not None:
+            rounds_out[0] = rounds_all
         for ev in self.sent:
             ev.record(self.sb)
         marks = []                                  # CUDA events around the stages of every round (self.trace)
         for r in range(rounds_all):
             bank = r & 1
-            off = r * self.round_bytes
-            ln = max(0, min(self.round_bytes, n - off))
             ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
             marks.append(ev)
             with torch.cuda.stream(self.sa):
                 self.sa.wait_event(self.sent[bank])
                 ev[0].record(self.sa)
-                if ln or (r == 0 and begin) or (r == rounds_all - 1 and end):
-                    src = fetch(off, ln, bank)
-                    self.hc.shard_extract(src, ln, bank, begin and r == 0, end and off + ln >= n, stream=self.sa.cuda_stream)
+                extract(r, bank)
                 ev[1].record(self.sa)
                 counts = self.hc.shard_pack(bank, stream=self.sa.cuda_stream)       # synchronises stream A
                 sc = torch.tensor(counts, dtype=torch.int64, device=self.dev)
@@ -203,6 +230,135 @@ class RecordExchange(object):
         for ev in marks:
             t[0] += ev[0].elapsed_time(ev[1]); t[1] += ev[2].elapsed_time(ev[3]); t[2] += ev[3].elapsed_time(ev[4])
         self.trace = {"rounds": rounds_all, "extract_ms": t[0], "exchange_ms": t[1], "restage_ms": t[2]}
+
+
+class ShareReader(object):
+    """Rank r's share of one file (jellyfish_b200.split.Share) read with pread, piece by piece, into two pinned host buffers:
+    host memory stays bounded whatever the size of the file (the seam, read whole, holds the lines walked back in front of
+    the share: one line for FASTA whose sequences are not wrapped).
+
+    Piece i covers the bytes from the end of piece i - 1 to start + (i + 1) * piece_bytes (the last one to the end of the
+    share), so every rank knows its number of pieces before it reads any.  A piece that is not the last one ends in front
+    of a trailing run of '\\r', which then begins the next piece: a device feed that ends on '\\r' takes the run for a line
+    end, where the byte behind it decides.  A run of CR_SLACK bytes or more there is refused (ValueError).
+
+    prefetch(i) reads piece i on a thread of its own, so that the disk or page-cache read overlaps the device work the
+    caller enqueues meanwhile; read(i) then only waits for it."""
+
+    CR_SLACK = 4096
+
+    def __init__(self, path, share, piece_bytes):
+        from . import _lib
+        self._lib = _lib.load()
+        self.fmt = share.fmt
+        self.share = share
+        self.piece = max(1, piece_bytes - self.CR_SLACK)
+        n = max(0, share.end - share.start)
+        self.n_pieces = (n + self.piece - 1) // self.piece
+        self.fd = os.open(path, os.O_RDONLY)
+        self.bufs = [None, None]
+        self.events = [None, None]
+        self.next_off = share.start
+        self._ahead = None                    # (piece, thread, [result or exception])
+        # without a seam the share's first piece begins the file's parse (JFGPU_FILE_BEGIN with the format flag)
+        self.first_begins = share.seam >= share.start
+
+    def seam(self):
+        """The seam's bytes (b"" when there is none)."""
+        s = self.share
+        return os.pread(self.fd, s.start - s.seam, s.seam) if s.seam < s.start else b""
+
+    def _load(self, i):
+        import ctypes as C
+        b = i & 1
+        if self.bufs[b] is None:
+            p = self._lib.jfgpu_host_alloc(self.piece + self.CR_SLACK)
+            if not p:
+                raise MemoryError("pinned host allocation failed")
+            self.bufs[b] = p
+        elif self.events[b] is not None:
+            self.events[b].synchronize()          # the copy of piece i - 2 out of this buffer is done
+        last = i == self.n_pieces - 1
+        stop = self.share.end if last else self.share.start + (i + 1) * self.piece
+        off = self.next_off
+        view = (C.c_char * (stop - off)).from_address(self.bufs[b])
+        got = os.preadv(self.fd, [view], off)
+        if got != stop - off:
+            raise IOError("short read of %d bytes at %d" % (stop - off, off))
+        n = got
+        if not last:
+            tail = bytes(memoryview(view)[max(0, n - self.CR_SLACK):n])
+            run = len(tail) - len(tail.rstrip(b"\r"))
+            if run == len(tail):
+                raise ValueError("a run of at least %d '\\r' bytes ends at byte %d, where the share is cut into pieces: "
+                                 "count this file with --split files" % (run, stop))
+            n -= run
+        self.next_off = off + n
+        return self.bufs[b], n, i == 0 and self.first_begins, last
+
+    def prefetch(self, i):
+        """Start reading piece i (the pieces before it have been read) on a thread; nothing when i is past the last."""
+        import threading
+        if i >= self.n_pieces or self._ahead is not None:
+            return
+        box = []
+
+        def run():
+            try:
+                box.append(self._load(i))
+            except BaseException as ex:            # handed to read(i)
+                box.append(ex)
+        t = threading.Thread(target=run, daemon=True)
+        self._ahead = (i, t, box)
+        t.start()
+
+    def read(self, i):
+        """-> (host pointer, n, begin, end) of piece i; pieces are read in order.  The buffer stays untouched until piece i + 2
+        is read or prefetched, which waits for the event release(i) records."""
+        if self._ahead is not None:
+            j, t, box = self._ahead
+            t.join()
+            self._ahead = None
+            if j == i:
+                if isinstance(box[0], BaseException):
+                    raise box[0]
+                return box[0]
+        return self._load(i)
+
+    def release(self, i, stream=None):
+        """Piece i has been copied out (on `stream`; None: synchronously)."""
+        if stream is None:
+            self.events[i & 1] = None
+            return
+        ev = torch.cuda.Event()
+        ev.record(stream)
+        self.events[i & 1] = ev
+
+    def close(self):
+        if self._ahead is not None:
+            self._ahead[1].join()
+            self._ahead = None
+        for p in self.bufs:
+            if p:
+                self._lib.jfgpu_host_free(p)
+        self.bufs = [None, None]
+        if self.fd >= 0:
+            os.close(self.fd)
+            self.fd = -1
+
+
+def fastq_cuts_agree(tallies, world, device):
+    """The FASTQ check of a split count: tallies = [(bytes, newlines) of this rank's share] per split FASTQ file, in the same
+    file order on every rank.  Gathers every rank's tallies and returns True when every non-empty share of every file
+    starts on a record (split.fastq_cuts_ok).  Every rank must call it."""
+    from .split import fastq_cuts_ok
+    if world == 1 or not tallies:
+        return True
+    mine = torch.tensor(tallies, dtype=torch.int64, device=device)
+    every = [torch.empty_like(mine) for _ in range(world)]
+    dist.all_gather(every, mine)
+    every = [t.tolist() for t in every]
+    return all(fastq_cuts_ok([every[r][f] for r in range(world)]) for f in range(len(tallies)))
 
 
 def default_batch_bytes(k):
@@ -253,7 +409,7 @@ class ShardedCounter(object):
             self.send = torch.empty((world, self.capacity * kw), dtype=torch.int64, device=self.dev)
             self.recv = torch.empty((world, self.capacity * kw), dtype=torch.int64, device=self.dev)
             self.counts = torch.zeros(world, dtype=torch.int64, device=self.dev)
-        self._host_stage = None
+        self._host_stage = self._piece_stage = None
         self._send2 = self._counts2 = self._sa = None
         # a dedicated (non-default) stream: its handle is passed to the engine so that kernels, tensor
         # ops and NCCL collectives are ordered on one stream (handle 0 would mean "engine stream")
@@ -272,9 +428,17 @@ class ShardedCounter(object):
         self.stream.synchronize()
 
     def _add_device_text(self, ptr, n, begin, end):
+        def extract(i, send, counts):
+            off = i * self.batch_bytes
+            ln = max(0, min(self.batch_bytes, n - off))
+            if ln:
+                self.backend.extract_route((ptr + off, ln), begin and off == 0, end and off + ln >= n, send, self.capacity, counts)
+        self._pipeline((n + self.batch_bytes - 1) // self.batch_bytes, extract)
+
+    def _pipeline(self, rounds, extract):
         """Two-stage software pipeline: the extraction of batch i+1 (stream A) overlaps the NVLink
-        exchange and the owner-side insertion of batch i (stream B).  Two send/count buffer sets."""
-        rounds = (n + self.batch_bytes - 1) // self.batch_bytes
+        exchange and the owner-side insertion of batch i (stream B).  Two send/count buffer sets.
+        extract(i, send, counts) buckets batch i on stream A (nothing when this rank has no text for it)."""
         t = torch.tensor([rounds], dtype=torch.int64, device=self.dev)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         rounds_all = int(t.item())        # every rank takes part in every exchange
@@ -292,14 +456,10 @@ class ShardedCounter(object):
             ev.record(sb)
 
         def launch_extract(i):
-            off = i * self.batch_bytes
-            ln = max(0, min(self.batch_bytes, n - off))
             with torch.cuda.stream(sa):
                 sa.wait_event(done_use[i & 1])           # the buffers of batch i-2 have been sent
                 cnts[i & 1].zero_()
-                if ln:
-                    self.backend.extract_route((ptr + off, ln), begin and off == 0, end and off + ln >= n,
-                                               sends[i & 1], self.capacity, cnts[i & 1])
+                extract(i, sends[i & 1], cnts[i & 1])
                 done_extract[i & 1].record(sa)
 
         if rounds_all:
@@ -345,6 +505,50 @@ class ShardedCounter(object):
                                            self.send, self.capacity, self.counts)
             exchange_and_insert(self.backend, self.world, self.send, self.counts, self.capacity, self.recv)
             off += ln
+
+    def piece_bytes(self):
+        """The most text one exchange round takes: a piece of a streamed share is never longer."""
+        return self.records.round_bytes if self.records is not None else self.batch_bytes
+
+    def add_pieces(self, reader, tally=None):
+        """Count a share of a file read piece by piece (ShareReader, pieces of at most piece_bytes()).  Every rank calls this
+        once per file, also with a share that is empty: every rank takes part in every exchange round.  The copy to the device
+        and the extraction of piece i + 1 run beside the exchange and insertion of piece i.  tally: a device int64 tensor
+        the newlines of the share are added to (jfgpu_count_newlines)."""
+        if self.world == 1:
+            for i in range(reader.n_pieces):
+                hptr, ln, begin, end = reader.read(i)
+                reader.prefetch(i + 1)
+                self.hc.add_text((hptr, ln), begin=begin, end=end, fmt=reader.fmt)
+                reader.release(i)
+            return
+        torch.cuda.current_stream(self.dev).synchronize()
+        if self.records is not None:
+            self.records.add_pieces(reader, tally)
+            return
+        if self._piece_stage is None:
+            self._piece_stage = [torch.empty(self.batch_bytes + 256, dtype=torch.uint8, device=self.dev) for _ in range(2)]
+        from . import _lib
+        import ctypes as C
+        lib = _lib.load()
+
+        def extract(i, send, counts):
+            if i >= reader.n_pieces:
+                return
+            hptr, ln, begin, end = reader.read(i)
+            dst = self._piece_stage[i & 1].data_ptr()
+            st = torch.cuda.current_stream(self.dev)
+            if ln and lib.jfgpu_memcpy_h2d(C.c_void_p(dst), C.c_void_p(hptr), ln, C.c_void_p(st.cuda_stream)):
+                raise RuntimeError("host to device copy failed")
+            reader.release(i, st)
+            reader.prefetch(i + 1)            # (read while the exchange of the piece before and this extraction run)
+            if tally is not None:
+                self.hc.count_newlines(dst, ln, tally.data_ptr(), stream=st.cuda_stream)
+            self.hc.extract_route(dst, ln, send.data_ptr(), self.capacity, counts.data_ptr(), begin=begin, end=end,
+                                  stream=st.cuda_stream, fmt=reader.fmt)
+        with torch.cuda.stream(self.stream):
+            self._pipeline(reader.n_pieces, extract)
+        self.stream.synchronize()
 
     def done(self):
         return self.hc.done()

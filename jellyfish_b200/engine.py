@@ -16,6 +16,16 @@ from . import _lib as L
 UINT64_MAX = (1 << 64) - 1
 
 
+def text_flags(begin, end, fmt=None):
+    """Feed flags of a piece of FASTA / FASTQ text.  fmt "fasta" or "fastq": the piece begins a share that starts at a line
+    start in the middle of a file of that format (include/jfgpu.h: JFGPU_FORMAT_FASTA / _FASTQ); None: the format is sniffed
+    from the first byte of the file."""
+    f = (L.FILE_BEGIN if begin else 0) | (L.FILE_END if end else 0)
+    if begin and fmt:
+        f |= {"fasta": L.FORMAT_FASTA, "fastq": L.FORMAT_FASTQ}[fmt]
+    return f
+
+
 class JellyfishError(RuntimeError):
     """Raised for any non-zero status of the engine (reference: std::runtime_error / err::die)."""
 
@@ -119,9 +129,10 @@ class HashCounter(object):
     def val_len(self):
         return self.info()["val_len"]
 
-    def add_text(self, data, begin=True, end=True):
-        """Count every k-mer of a buffer of FASTA text held in host memory (bytes or a pointer/size pair)."""
-        flags = (L.FILE_BEGIN if begin else 0) | (L.FILE_END if end else 0)
+    def add_text(self, data, begin=True, end=True, fmt=None):
+        """Count every k-mer of a buffer of FASTA text held in host memory (bytes or a pointer/size pair).  fmt: see
+        text_flags."""
+        flags = text_flags(begin, end, fmt)
         if isinstance(data, tuple):
             ptr, n = data
         else:
@@ -129,9 +140,9 @@ class HashCounter(object):
             ptr, n = C.cast(C.c_char_p(buf), C.c_void_p), len(buf)
         self._check(self._lib.jfgpu_feed(self._h, ptr, n, flags))
 
-    def add_device_text(self, dev_ptr, n, begin=True, end=True, stream=None, sam=False):
+    def add_device_text(self, dev_ptr, n, begin=True, end=True, stream=None, sam=False, fmt=None):
         """Same with the text already in device memory (e.g. a torch uint8 tensor's data_ptr()); sam=True: SAM text."""
-        flags = (L.FILE_BEGIN if begin else 0) | (L.FILE_END if end else 0) | (L.FORMAT_SAM if sam else 0)
+        flags = text_flags(begin, end, fmt) | (L.FORMAT_SAM if sam else 0)
         self._check(self._lib.jfgpu_feed_device(self._h, C.c_void_p(dev_ptr), n, flags, C.c_void_p(stream or 0)))
 
     def add_files(self, paths, chunk=64 << 20):
@@ -184,8 +195,27 @@ class HashCounter(object):
                         break
                     cur = nxt
 
-    def extract_route(self, dev_ptr, n, keys_ptr, capacity, counts_ptr, begin=True, end=True, stream=None):
-        flags = (L.FILE_BEGIN if begin else 0) | (L.FILE_END if end else 0)
+    def seam(self, dev_ptr, n, fmt=None, begin=True, stream=None):
+        """Parse device text [dev_ptr, dev_ptr + n) without counting it: the next feed without `begin` continues where it
+        ends (include/jfgpu.h: jfgpu_seam).  The text in front of a share of a file, so that the share is counted as the
+        whole file would count it."""
+        self._check(self._lib.jfgpu_seam(self._h, C.c_void_p(dev_ptr), n, text_flags(begin, False, fmt), C.c_void_p(stream or 0)))
+
+    def seam_text(self, data, fmt=None, begin=True):
+        """seam() of text in host memory (bytes or a pointer/size pair): jfgpu_seam_host."""
+        if isinstance(data, tuple):
+            ptr, n = data
+        else:
+            buf = bytes(data)
+            ptr, n = C.cast(C.c_char_p(buf), C.c_void_p), len(buf)
+        self._check(self._lib.jfgpu_seam_host(self._h, ptr, n, text_flags(begin, False, fmt)))
+
+    def count_newlines(self, dev_ptr, n, count_ptr, stream=None):
+        """Add the '\\n' bytes of device text to the device uint64 at count_ptr (stream-ordered: jfgpu_count_newlines)."""
+        self._check(self._lib.jfgpu_count_newlines(self._h, C.c_void_p(dev_ptr), n, C.c_void_p(count_ptr), C.c_void_p(stream or 0)))
+
+    def extract_route(self, dev_ptr, n, keys_ptr, capacity, counts_ptr, begin=True, end=True, stream=None, fmt=None):
+        flags = text_flags(begin, end, fmt)
         self._check(self._lib.jfgpu_extract_route(self._h, C.c_void_p(dev_ptr), n, flags, C.c_void_p(keys_ptr),
                                                   capacity, C.c_void_p(counts_ptr), C.c_void_p(stream or 0)))
 
@@ -206,8 +236,8 @@ class HashCounter(object):
     def shard_round_bytes(self):
         return self._lib.jfgpu_shard_round_bytes(self._h)
 
-    def shard_extract(self, dev_ptr, n, bank, begin=True, end=True, stream=None):
-        flags = (L.FILE_BEGIN if begin else 0) | (L.FILE_END if end else 0)
+    def shard_extract(self, dev_ptr, n, bank, begin=True, end=True, stream=None, fmt=None):
+        flags = text_flags(begin, end, fmt)
         self._check(self._lib.jfgpu_shard_extract(self._h, C.c_void_p(dev_ptr), n, flags, bank, C.c_void_p(stream or 0)))
 
     def shard_pack(self, bank, stream=None):
@@ -418,8 +448,11 @@ class BloomCounter(object):
     def add_files(self, paths):
         self.hc.add_files(paths)
 
-    def add_text(self, data, begin=True, end=True):
-        self.hc.add_text(data, begin=begin, end=end)
+    def add_text(self, data, begin=True, end=True, fmt=None):
+        self.hc.add_text(data, begin=begin, end=end, fmt=fmt)
+
+    def seam_text(self, data, fmt=None, begin=True):
+        self.hc.seam_text(data, fmt=fmt, begin=begin)
 
     def info(self):
         return self.hc.bloom_info()
