@@ -180,6 +180,19 @@ int  jfgpu_feed(jfgpu_handle h, const char* bytes, size_t n, uint32_t flags);
  * `stream` is a cudaStream_t (NULL = the engine's own stream). */
 int  jfgpu_feed_device(jfgpu_handle h, const void* dev_bytes, size_t n, uint32_t flags, void* stream);
 
+/* -- SAM and BAM records turned into FASTQ without counting them (no reference analogue: the multi-GPU driver routes the
+ *    FASTQ of a batch of whole records as a FASTQ file of its own, JFGPU_FILE_BEGIN | JFGPU_FILE_END | JFGPU_FORMAT_FASTQ,
+ *    since no k-mer spans two reads).  The input is what jfgpu_feed (on_device = 0) or jfgpu_feed_device (on_device = 1,
+ *    SAM only, 16-byte aligned) takes with JFGPU_FORMAT_SAM / _BAM: the same flags, the same carry of an incomplete last
+ *    line, header field or record to the next call, the same JFGPU_ERR_FORMAT messages and byte offsets.  The FASTQ of the
+ *    records completed by this call, "@\n SEQ \n+\n QUAL \n" each, is written to dev_out (device memory, any alignment)
+ *    and *out_len receives its size; it is at most twice the bytes given plus those carried in, and JFGPU_ERR_ARG is returned
+ *    when it would pass out_cap.  Nothing is counted and the text feeds are not disturbed: the staged file keeps its own
+ *    carry, so jfgpu_feed, jfgpu_extract_route and jfgpu_shard_extract may run between two calls.  The call returns when the
+ *    FASTQ is in dev_out; it runs after the work queued on `stream` (NULL = the engine's own stream). */
+int  jfgpu_sam_stage(jfgpu_handle h, const void* bytes, size_t n, uint32_t flags, int on_device, void* dev_out, size_t out_cap,
+                     size_t* out_len, void* stream);
+
 /* -- the seam in front of a share of a file (no reference analogue: the reference reads every file whole).  Parse the text
  *    [dev_bytes, dev_bytes + n) and keep only what a feed leaves to the next one: the parser state and the last symbols
  *    (the k-1 base seam).  Nothing is counted: no table, route bucket or Bloom structure is touched and the statistics do not

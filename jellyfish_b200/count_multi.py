@@ -22,6 +22,14 @@ exactly the positions r*size/N ... (r+1)*size/N - 1.  (`jellyfish merge` on the 
 same records: jellyfish/merge_files.cc:45-176.)  -m takes 1..128; k > 64 (32-byte keys) is routed by the key exchange
 on 2, 4 or 8 GPUs, with 64 MB batches.
 
+`--sam PATH` (may be given several times; read after the positional files) counts the reads of SAM text, gzip'd SAM and
+BAM files, each record's SEQ with its QUAL as one FASTQ read, as the single-GPU `count --sam` does
+(jellyfish_b200/split_sam.py).  With `--split auto`, SAM text is cut at line starts and BAM at a BGZF block and the first
+record behind it; every rank inflates its own blocks on a pool of threads.  Each piece is turned into FASTQ on the device
+(jfgpu_sam_stage) and routed as FASTQ.  A BAM rank's records must end exactly where the next rank's start: when they do
+not, every rank clears its table and counts whole files, with a note on stderr.  gzip'd SAM and pipes are counted whole by
+one rank; CRAM is refused.
+
 Bloom structures (k <= 64) take the key exchange: `--bc FILE` is loaded whole by every rank and tested before a k-mer is
 routed; `--bf-size N` (the GLOBAL expected number of k-mers) gives every rank a filter for its share, applied by the
 owner after the exchange, where every occurrence of a k-mer arrives.
@@ -29,11 +37,14 @@ owner after the exchange, where every occurrence of a k-mer arrives.
 import argparse
 import os
 import sys
+import time
 
 import torch
 import torch.distributed as dist
 
-from .distributed import ShardedCounter, ShareReader, concat_shards, fastq_cuts_agree
+from . import split_sam
+from .engine import JellyfishError
+from .distributed import ShardedCounter, ShareReader, all_ranks_ok, concat_shards, fastq_cuts_agree
 from .split import plan_file, splittable
 
 
@@ -101,7 +112,62 @@ def count_split(sc, files, rank, world, k):
     return fastq_cuts_agree(tallies, world, "cuda")
 
 
-def main(argv=None):
+def _count_sam_reader(sc, path, reader, tolerant=False):
+    """A corrupt or truncated BGZF block (found while inflating, on the reader's thread) is a one-line error."""
+    try:
+        return sc.add_sam_pieces(reader, tolerant)
+    except ValueError as ex:
+        raise SystemExit("%s: %s" % (path, ex))
+    finally:
+        reader.close()
+        sc.sam_inflate_s += getattr(reader, "inflate_s", 0.0)
+
+
+def _whole_sam(sc, path, owner):
+    try:
+        reader = split_sam.whole_reader(path, owner, sc.sam_piece_bytes())
+    except ValueError as ex:
+        raise SystemExit("%s: %s" % (path, ex))
+    _count_sam_reader(sc, path, reader)
+
+
+def count_sam_files(sc, sams, rank, world):
+    """--split files (and the fall-back): rank r counts the SAM / BAM files sams[r::world] whole."""
+    t0 = time.perf_counter()
+    for i, path in enumerate(sams):
+        _whole_sam(sc, path, i % world == rank)
+    sc.sam_wall_s += time.perf_counter() - t0
+
+
+def count_sam_split(sc, sams, rank, world):
+    """--split auto for --sam files: SAM text and BAM split among the ranks, anything else counted whole by rank i % world.
+    Returns False on this rank when one of its shares could not be counted on its own (a BAM record chain that does not end
+    where the next share starts): the table then holds a wrong count and must be cleared."""
+    ok = True
+    t0 = time.perf_counter()
+    for i, path in enumerate(sams):
+        k = split_sam.kind(path) if splittable(path) else "pipe"
+        if k == "cram":
+            raise SystemExit("CRAM input is not supported ('%s')" % path)
+        if k not in ("sam", "bam"):
+            if k is not None:
+                _whole_sam(sc, path, i % world == rank)
+            continue
+        try:
+            kind_, share = split_sam.plan_file(path, rank, world, k)
+            if kind_ == "sam":
+                reader = split_sam.SamShareReader(path, share, sc.sam_piece_bytes())
+            else:
+                reader = split_sam.BamShareReader(path, share, sc.sam_piece_bytes())
+        except ValueError as ex:
+            raise SystemExit("%s: %s" % (path, ex))
+        ok = _count_sam_reader(sc, path, reader, tolerant=True) and ok
+    sc.sam_wall_s += time.perf_counter() - t0
+    return ok
+
+
+def parse_args(argv=None):
+    """The command line, checked as the single-GPU command checks it (exits on an error)."""
     ap = argparse.ArgumentParser(prog="jellyfish_b200.count_multi", description=__doc__.split("\n")[0])
     ap.add_argument("-m", "--mer-len", type=int, required=True)
     ap.add_argument("-s", "--size", type=_size, required=True, help="GLOBAL table size (as for jellyfish count)")
@@ -118,16 +184,24 @@ def main(argv=None):
     ap.add_argument("--keep-shards", action="store_true")
     ap.add_argument("--split", choices=("auto", "files"), default="auto",
                     help="auto: split every file among the ranks; files: give rank r the whole files files[r::N]")
-    ap.add_argument("files", nargs="+")
+    ap.add_argument("--sam", action="append", default=[], metavar="PATH",
+                    help="SAM, gzip'd SAM or BAM file to count (may be given several times)")
+    ap.add_argument("files", nargs="*")
     a = ap.parse_args(argv)
     # the single-GPU command's checks (count_main.cc:196-197 and the k <= 64 scope of every Bloom structure)
     if a.bf_size and a.bc:
         sys.stderr.write("Error: Switches [--bf-size] and [--bc] conflict\n")
         sys.exit(1)
+    if not a.files and not a.sam:
+        ap.error("no input file: give sequence files or --sam")
     if a.mer_len > 64 and (a.bf_size or a.bc):
         sys.stderr.write("Error: --bf-size and --bc take mer lengths up to 64\n")
         sys.exit(1)
+    return a
 
+
+def main(argv=None):
+    a = parse_args(argv)
     rank, world = int(os.environ.get("RANK", "0")), int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", rank))
     torch.cuda.set_device(local)
@@ -135,16 +209,42 @@ def main(argv=None):
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         os.environ.setdefault("NCCL_MAX_CTAS", "16")      # K1 leaves 16 SMs to the exchange that runs beside it
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+    run(a, argv, rank, world, local)
+
+
+def run(a, argv, rank, world, local):
+    """Count and write the output on this rank of an initialised process group (world 1: none); an engine error is a
+    one-line message and exit status 1."""
+    try:
+        _count(a, argv, rank, world, local)
+    except JellyfishError as ex:
+        sys.stderr.write("count_multi: %s\n" % ex)
+        sys.exit(1)
+
+
+def _count(a, argv, rank, world, local):
     sc = ShardedCounter(a.size, a.counter_len, k=a.mer_len, canonical=a.canonical, rank=rank, world=world, device=local,
                         reprobes=a.reprobes, bf_size=a.bf_size, bf_fp=a.bf_fp, bc=a.bc)
+    sc.sam_inflate_s = sc.sam_wall_s = 0.0
     if a.split == "files":
         count_files(sc, a.files, rank, world)
-    elif not count_split(sc, a.files, rank, world, a.mer_len):
-        if rank == 0:
-            sys.stderr.write("count_multi: a FASTQ share does not start on a record; counting whole files per rank instead\n")
-        sc.hc.clear()
-        count_files(sc, a.files, rank, world)
+        count_sam_files(sc, a.sam, rank, world)
+    else:
+        fastq_ok = count_split(sc, a.files, rank, world, a.mer_len)
+        sam_ok = all_ranks_ok(count_sam_split(sc, a.sam, rank, world), world, "cuda")
+        if not (fastq_ok and sam_ok):
+            if rank == 0:
+                what = "a FASTQ share does not start on a record" if not fastq_ok else \
+                    "a SAM/BAM share could not be counted on its own (a BAM record chain does not meet the next share)"
+                sys.stderr.write("count_multi: %s; counting whole files per rank instead\n" % what)
+            sc.hc.clear()
+            count_files(sc, a.files, rank, world)
+            count_sam_files(sc, a.sam, rank, world)
     st = sc.done()
+    if a.sam:
+        # (read by scripts/sam_multi_bench.py)
+        sys.stderr.write("count_multi: rank %d --sam times: inflate_s %.4f transcode_route_s %.4f sam_wall_s %.4f\n"
+                         % (rank, sc.sam_inflate_s, sc.sam_device_s, sc.sam_wall_s))
     cmdline = ["count_multi"] + (argv if argv is not None else sys.argv[1:])
     sc.hc.dump("%s.%d" % (a.output, rank), lower=a.lower_count, upper=a.upper_count, out_counter_len=a.out_counter_len, cmdline=cmdline)
     if world > 1:

@@ -60,6 +60,8 @@ template<typename T> struct HostBuf {            // pinned host memory
   T* p = nullptr;
   HostBuf() = default;
   HostBuf(const HostBuf&) = delete;
+  HostBuf(HostBuf&& o) noexcept : p(o.p) { o.p = nullptr; }
+  HostBuf& operator=(HostBuf&& o) noexcept { if(this != &o) { reset(); std::swap(p, o.p); } return *this; }
   ~HostBuf() { reset(); }
   cudaError_t alloc(size_t bytes) { reset(); const cudaError_t c = cudaHostAlloc((void**)&p, bytes, cudaHostAllocDefault); if(c) p = nullptr; return c; }
   void reset() { if(p) cudaFreeHost(p); p = nullptr; }
@@ -250,6 +252,11 @@ struct jfgpu_engine {
     uint64_t bam_skip = 0;                          // bytes of header text or reference name still to pass over
     uint64_t done_off = 0;                          // bytes of the file in front of the next batch (messages)
   } sam;
+  // jfgpu_sam_stage: the file being staged keeps its own SamState (swapped into `sam` for the length of a call), so that the
+  // feeds and routings between two stage calls do not reset its carry; a batch's FASTQ is appended to the caller's buffer
+  SamState sam_staged;
+  uint8_t* stage_out = nullptr;
+  size_t stage_out_cap = 0, stage_out_len = 0;
 };
 
 namespace {
@@ -1537,6 +1544,11 @@ void jfgpu_destroy(jfgpu_handle e) {
   delete e;                      // (every buffer, event and stream is released by its owner, the streams last)
 }
 
+static void sam_begin(jfgpu_engine::SamState& s, uint32_t form) {
+  s.form = form; s.tail.clear(); s.tail_dev_len = 0;
+  s.bam_phase = 0; s.bam_refs = 0; s.bam_skip = 0; s.done_off = 0;
+}
+
 static int begin_feed(jfgpu_engine* e, uint32_t flags, int first_byte, cudaStream_t st) {
   if((flags & TEXT_FLAGS) == TEXT_FLAGS || ((flags & TEXT_FLAGS) && (flags & SAM_FLAGS)))
     return fail(e, JFGPU_ERR_ARG, "JFGPU_FORMAT_FASTA, _FASTQ, _SAM and _BAM exclude each other");
@@ -1547,8 +1559,7 @@ static int begin_feed(jfgpu_engine* e, uint32_t flags, int first_byte, cudaStrea
     if(!form && !(flags & TEXT_FLAGS) && first_byte >= 0 && first_byte != '>' && first_byte != '@') return fail(e, JFGPU_ERR_FORMAT, "Unsupported format");
     // SAM and BAM records reach the extraction kernels as 4-line FASTQ
     e->format = form || (flags & JFGPU_FORMAT_FASTQ) || (!(flags & JFGPU_FORMAT_FASTA) && first_byte == '@') ? 1 : 0;
-    e->sam.form = form; e->sam.tail.clear(); e->sam.tail_dev_len = 0;
-    e->sam.bam_phase = 0; e->sam.bam_refs = 0; e->sam.bam_skip = 0; e->sam.done_off = 0;
+    sam_begin(e->sam, form);
     int rc = reset_carry(e, st);
     if(rc) return rc;
     e->in_file = true;
@@ -1651,6 +1662,13 @@ static int sam_run(jfgpu_engine* e, cudaStream_t st, const uint8_t* dev, size_t 
   }
   *used = s.form == 2 ? n : (size_t)r.consumed;
   if(!r.out_bytes) return JFGPU_OK;
+  if(e->stage_out) {                          // jfgpu_sam_stage: the FASTQ goes to the caller, nothing is counted
+    if(r.out_bytes > e->stage_out_cap - e->stage_out_len)
+      return fail(e, JFGPU_ERR_ARG, "jfgpu_sam_stage: the FASTQ of the input does not fit out_cap (" + std::to_string(e->stage_out_cap) + " bytes)");
+    CUDA_OK(e, cudaMemcpyAsync(e->stage_out + e->stage_out_len, s.out.p, r.out_bytes, cudaMemcpyDeviceToDevice, st));
+    e->stage_out_len += r.out_bytes;
+    return JFGPU_OK;
+  }
   if((e->p.allow_regrow || e->spill_fn) && e->tab.slots.p) {            // as jfgpu_feed: a failed insertion regrows first
     CUDA_OK(e, cudaMemcpyAsync(e->h_stats + STAT_FAILED, e->stats.as<unsigned long long>() + STAT_FAILED, 8, cudaMemcpyDeviceToHost, e->cs));
     CUDA_OK(e, cudaStreamSynchronize(e->cs));
@@ -1859,6 +1877,50 @@ static int sam_feed(jfgpu_engine* e, const void* data, size_t n, uint32_t flags,
   e->bytes_fed += n;
   if(e->tab.slots.p) { rc = check_after_batches(e); if(rc) return rc; }
   return end_feed(e, flags, st);
+}
+
+// The transcode of a SAM or BAM file without counting: sam_feed's walk, with sam_run appending every batch's FASTQ to the
+// caller's buffer.  The file's carry lives in sam_staged between calls.
+static int sam_stage_run(jfgpu_engine* e, const void* data, size_t n, uint32_t flags, bool device, cudaStream_t st) {
+  jfgpu_engine::SamState& s = e->sam;
+  const uint32_t form = flags & JFGPU_FORMAT_BAM ? 2 : flags & JFGPU_FORMAT_SAM ? 1 : 0;
+  if(flags & TEXT_FLAGS) return fail(e, JFGPU_ERR_ARG, "jfgpu_sam_stage takes SAM or BAM input only");
+  if((flags & SAM_FLAGS) == SAM_FLAGS) return fail(e, JFGPU_ERR_ARG, "JFGPU_FORMAT_SAM and JFGPU_FORMAT_BAM exclude each other");
+  if(flags & JFGPU_FILE_BEGIN) {
+    if(!form) return fail(e, JFGPU_ERR_ARG, "jfgpu_sam_stage: JFGPU_FILE_BEGIN needs JFGPU_FORMAT_SAM or JFGPU_FORMAT_BAM");
+    sam_begin(s, form);
+  } else if(!s.form) {
+    return fail(e, JFGPU_ERR_STATE, "jfgpu_sam_stage: no SAM or BAM file is being staged (JFGPU_FILE_BEGIN)");
+  } else if(form && form != s.form) {
+    return fail(e, JFGPU_ERR_ARG, "the format flag differs from the one the file began with");
+  }
+  if(device && s.form == 2) return fail(e, JFGPU_ERR_ARG, "BAM input is taken from host memory only");
+  int rc = sam_alloc(e);
+  if(rc) return rc;
+  const bool end = flags & JFGPU_FILE_END;
+  if(device) rc = sam_feed_device(e, (const uint8_t*)data, n, end, st);
+  else if(s.form == 2) rc = bam_feed_host(e, (const char*)data, n, end);
+  else rc = sam_feed_host(e, (const char*)data, n, end);
+  if(!rc) CUDA_OK(e, cudaStreamSynchronize(device ? st : e->cs));
+  if(rc || end) s.form = 0;                 // (a failed file is not continued)
+  return rc;
+}
+
+int jfgpu_sam_stage(jfgpu_handle e, const void* bytes, size_t n, uint32_t flags, int on_device, void* dev_out, size_t out_cap,
+                    size_t* out_len, void* stream) {
+  if(!e || (n && !bytes) || !dev_out || !out_len) return JFGPU_ERR_ARG;
+  *out_len = 0;
+  cudaSetDevice(e->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
+  // host input runs on the engine's streams: the work the caller has queued on `stream` (e.g. on dev_out) comes first
+  if(!on_device && stream) CUDA_OK(e, cudaStreamSynchronize(st));
+  std::swap(e->sam, e->sam_staged);
+  e->stage_out = (uint8_t*)dev_out; e->stage_out_cap = out_cap; e->stage_out_len = 0;
+  const int rc = sam_stage_run(e, bytes, n, flags, on_device != 0, st);
+  *out_len = e->stage_out_len;
+  e->stage_out = nullptr; e->stage_out_cap = e->stage_out_len = 0;
+  std::swap(e->sam, e->sam_staged);
+  return rc;
 }
 
 int jfgpu_feed_device(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_t flags, void* stream) {

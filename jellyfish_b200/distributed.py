@@ -14,6 +14,7 @@ ordering of the shard files) is plain torch.distributed code and is exercised on
 tests/test_distributed_cpu.py through the `RouteBackend` seam below.
 """
 import os
+import time
 
 import torch
 import torch.distributed as dist
@@ -170,6 +171,21 @@ class RecordExchange(object):
                 self.hc.count_newlines(src, ln, tally.data_ptr(), stream=self.sa.cuda_stream)
             self.hc.shard_extract(src, ln, bank, begin, end, stream=self.sa.cuda_stream, fmt=reader.fmt)
         self._run(reader.n_pieces, extract)
+
+    def add_sam_pieces(self, n_pieces, stage):
+        """SAM / BAM pieces: stage(i, stream) transcodes piece i into FASTQ of whole records in device memory -> (pointer,
+        bytes), which round i extracts as a FASTQ file of its own.  Both run on the host thread while stream B exchanges
+        and restages round i - 1.  Returns the host time of the stages and extractions (both synchronise)."""
+        spent = [0.0]
+
+        def extract(r, bank):
+            t0 = time.perf_counter()
+            ptr, n = stage(r, self.sa)
+            if n:
+                self.hc.shard_extract(ptr, n, bank, True, True, stream=self.sa.cuda_stream, fmt="fastq")
+            spent[0] += time.perf_counter() - t0
+        self._run(n_pieces, extract)
+        return spent[0]
 
     def _rounds(self, n, begin, end, fetch):
         rounds = (n + self.round_bytes - 1) // self.round_bytes if n else 0
@@ -361,6 +377,15 @@ def fastq_cuts_agree(tallies, world, device):
     return all(fastq_cuts_ok([every[r][f] for r in range(world)]) for f in range(len(tallies)))
 
 
+def all_ranks_ok(ok, world, device):
+    """True when `ok` holds on every rank (one all-reduce; every rank must call it)."""
+    if world == 1:
+        return bool(ok)
+    t = torch.tensor([1 if ok else 0], dtype=torch.int64, device=device)
+    dist.all_reduce(t, op=dist.ReduceOp.MIN)
+    return bool(t.item())
+
+
 def default_batch_bytes(k):
     """Text per exchange round of the key exchange.  Its three buffers (send, the second send bank, recv) take about
     8 * key_words * 1.25 bytes per batch byte each: 256 MB batches for k <= 64 (one or two key words), 64 MB for four-word
@@ -411,6 +436,10 @@ class ShardedCounter(object):
             self.counts = torch.zeros(world, dtype=torch.int64, device=self.dev)
         self._host_stage = self._piece_stage = None
         self._send2 = self._counts2 = self._sa = None
+        self._sam_out = None
+        # host time of transcoding and routing the --sam pieces (jfgpu_sam_stage and the extraction, both synchronised;
+        # one rank: transcoding and counting them)
+        self.sam_device_s = 0.0
         # a dedicated (non-default) stream: its handle is passed to the engine so that kernels, tensor
         # ops and NCCL collectives are ordered on one stream (handle 0 would mean "engine stream")
         self.stream = torch.cuda.Stream(device=self.dev)
@@ -549,6 +578,69 @@ class ShardedCounter(object):
         with torch.cuda.stream(self.stream):
             self._pipeline(reader.n_pieces, extract)
         self.stream.synchronize()
+
+    def sam_piece_bytes(self):
+        """Input bytes of a SAM / BAM piece.  Its FASTQ is at most twice the piece plus the line or record the engine carries
+        in from the piece before (at most batch_bytes / 2), and it holds at most half as many k-mers as bytes: so the FASTQ
+        of a piece holds no more k-mers than piece_bytes() of text."""
+        return max(1, min(self.piece_bytes(), self.batch_bytes) // 2)
+
+    def add_sam_pieces(self, reader, tolerant=False):
+        """Count a SAM or BAM file, or a share of one, read piece by piece (jellyfish_b200.split_sam readers, pieces of at most
+        sam_piece_bytes()).  Every rank calls this once per file, also with no pieces.  Each piece is transcoded into FASTQ
+        of whole records (jfgpu_sam_stage) and routed as a FASTQ file of its own.  Piece i + 1 is read and inflated on the
+        reader's thread while piece i is transcoded, routed and exchanged.  The record exchange also transcodes and extracts
+        piece i + 1 while its stream B exchanges piece i; the key exchange does not: its pipeline stages piece i + 1 (host
+        synchronous) between the count exchange and the payload exchange of piece i.  tolerant: a malformed piece (JFGPU_ERR_FORMAT, e.g. a BAM share whose
+        record chain does not end at the next share's start) ends this reader's work, and False is returned; the other
+        ranks go on with the exchange rounds.  Returns True otherwise."""
+        from .engine import JellyfishError
+        from . import _lib as L
+        if self.world == 1:
+            for i in range(reader.n_pieces):
+                data, begin, end = reader.read(i)
+                reader.prefetch(i + 1)
+                t0 = time.perf_counter()
+                self.hc.add_sam_text(data, begin=begin, end=end, bam=reader.bam)
+                self.sam_device_s += time.perf_counter() - t0
+                reader.release(i)
+            return True
+        torch.cuda.current_stream(self.dev).synchronize()
+        if self._sam_out is None:
+            self._sam_cap = 2 * (self.sam_piece_bytes() + self.batch_bytes // 2) + 64
+            self._sam_out = [torch.empty(self._sam_cap, dtype=torch.uint8, device=self.dev) for _ in range(2)]
+        ok = [True]
+
+        def stage(i, st):
+            out = self._sam_out[i & 1].data_ptr()
+            if i >= reader.n_pieces or not ok[0]:
+                return out, 0
+            try:
+                data, begin, end = reader.read(i)
+                reader.prefetch(i + 1)       # (inflated while this piece is transcoded and the piece before is exchanged)
+                n = self.hc.sam_stage(data, out, self._sam_cap, begin=begin, end=end, bam=reader.bam, stream=st.cuda_stream)
+                reader.release(i)
+            except JellyfishError as ex:
+                if not tolerant or ex.code != L.ERR_FORMAT:
+                    raise
+                ok[0] = False
+                return out, 0
+            return out, n
+        if self.records is not None:
+            self.sam_device_s += self.records.add_sam_pieces(reader.n_pieces, stage)
+            return ok[0]
+
+        def extract(i, send, counts):
+            t0 = time.perf_counter()
+            ptr, n = stage(i, torch.cuda.current_stream(self.dev))
+            if n:
+                self.hc.extract_route(ptr, n, send.data_ptr(), self.capacity, counts.data_ptr(), begin=True, end=True,
+                                      stream=torch.cuda.current_stream(self.dev).cuda_stream, fmt="fastq")
+            self.sam_device_s += time.perf_counter() - t0
+        with torch.cuda.stream(self.stream):
+            self._pipeline(reader.n_pieces, extract)
+        self.stream.synchronize()
+        return ok[0]
 
     def done(self):
         return self.hc.done()

@@ -195,6 +195,25 @@ class HashCounter(object):
                         break
                     cur = nxt
 
+    def sam_stage(self, data, out_ptr, out_cap, begin=True, end=True, bam=False, stream=None):
+        """Turn SAM text or (bam=True) an inflated BAM stream into FASTQ without counting it (include/jfgpu.h:
+        jfgpu_sam_stage).  data: bytes or a (pointer, size) pair in host memory, or ("device", pointer, size) for SAM text in
+        device memory.  The FASTQ of the records this call completes goes to the device buffer at out_ptr (out_cap bytes);
+        returns its size.  A file may come in any number of pieces, cut anywhere, as for add_sam_text."""
+        flags = (L.FILE_BEGIN if begin else 0) | (L.FILE_END if end else 0) | (L.FORMAT_BAM if bam else L.FORMAT_SAM)
+        on_device = isinstance(data, tuple) and len(data) == 3
+        if on_device:
+            ptr, n = C.c_void_p(data[1]), data[2]
+        elif isinstance(data, tuple):
+            ptr, n = C.c_void_p(data[0]) if isinstance(data[0], int) else data[0], data[1]
+        else:
+            buf = bytes(data)
+            ptr, n = C.cast(C.c_char_p(buf), C.c_void_p), len(buf)
+        out_len = C.c_size_t(0)
+        self._check(self._lib.jfgpu_sam_stage(self._h, ptr, n, flags, int(on_device), C.c_void_p(out_ptr), out_cap, C.byref(out_len),
+                                              C.c_void_p(stream or 0)))
+        return out_len.value
+
     def seam(self, dev_ptr, n, fmt=None, begin=True, stream=None):
         """Parse device text [dev_ptr, dev_ptr + n) without counting it: the next feed without `begin` continues where it
         ends (include/jfgpu.h: jfgpu_seam).  The text in front of a share of a file, so that the share is counted as the
