@@ -476,7 +476,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
         const bool in_seq = a.format == 1 ? (a.tile_state[t] == 1) : (a.tile_state[t] != ST_H);
         if(lane == 0 && in_seq && idx0 < k - 1 && !sm.halo_break) {
           // pathological input (very short lines / long runs of blank lines): exact slow path
-          if(a.format == 1) backfill_fastq<PREK>(a.in, a.n_look, a.carry_in, h, PREK, sm.pre);
+          if(a.format == 1) backfill_fastq<PREK>(a.in, a.n_look, a.carry_in, h, PREK, sm.pre, a.min_qual, a.n_back);
           else backfill_symbols<PREK>(a.in, a.n_look, a.carry_in, h, -2, PREK, sm.pre, a.min_qual != 0);
         }
       }
@@ -497,7 +497,9 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
     // hand the parser state to the next batch
     if(t == a.n_tiles - 1 && warp == 1) {
       uint8_t* cs = a.carry_out->sym;
-      const bool not_seq = a.format == 1 ? (a.tile_state[t] != 1) : (a.tile_state[t] == ST_H);
+      // (FASTQ: the backfill reads the line that holds byte n - 1, so the batch has to end in a sequence line; one that ends
+      // in a header, '+' or quality line hands over the stream, whose last reset is that header's or comes before the next)
+      const bool not_seq = a.format == 1 ? (a.tile_state[t] != 1 || (sm.total_state & 3u) != 1u) : (a.tile_state[t] == ST_H);
       if(nsym >= (uint32_t)PREK || t == 0 || sm.halo_break || not_seq) {
 #pragma unroll
         for(int q = 0; q < PREK / 32; ++q) {                // the last PREK symbols of the stream
@@ -506,7 +508,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
           cs[lane + 32 * q] = (uint8_t)(((sm.brk[s >> 5] >> (s & 31u)) & 1u) ? SYM_BREAK : code);
         }
       } else if(lane == 0) {
-        if(a.format == 1) backfill_fastq<PREK>(a.in, a.n_look, a.carry_in, (long long)n, PREK, cs);
+        if(a.format == 1) backfill_fastq<PREK>(a.in, a.n_look, a.carry_in, (long long)n, PREK, cs, a.min_qual, a.n_back);
         else backfill_symbols<PREK>(a.in, a.n_look, a.carry_in, (long long)n, -2, PREK, cs, a.min_qual != 0);
       }
       if(lane == 0) a.carry_out->state = a.format == 1 ? (sm.total_state | (a.in[n - 1] == '\n' ? 4u : 0u)) : sm.total_state;

@@ -284,10 +284,21 @@ __device__ void backfill_symbols(const uint8_t* in, uint64_t n, const Carry* cin
 
 // FASTQ slow path: a sequence line is never continued from another line, so the symbols before
 // `end` are those of the same line (back to its '\n'), then a reset; before the batch start the
-// previous batch's carry continues the line.
+// previous batch's carry continues the line.  The caller knows that `end` lies in a sequence line.
+// -Q (min_qual != 0): the line is read as K1's per-byte path reads it -- a '\r' resets, and so does a base whose quality
+// byte (two lines further down, same column; the line start is looked for at most n_back bytes before the batch) is
+// below min_qual as a signed char, or lies at or past n.  Out of line: a cold path that, inlined, made K1 slower.
 template<int CPRE = PRE>
-__device__ void backfill_fastq(const uint8_t* in, uint64_t n, const Carry* cin, long long end, int need, uint8_t* out) {
+__device__ __noinline__ void backfill_fastq(const uint8_t* in, uint64_t n, const Carry* cin, long long end, int need, uint8_t* out,
+                               uint32_t min_qual = 0, uint64_t n_back = 0) {
   for(int i = 0; i < need; ++i) out[i] = SYM_BREAK;
+  long long qoff = -1;                 // -Q: the quality of the byte at p is in[p + qoff]; -1: none in the text
+  if(min_qual && end > 0) {
+    long long sl = end - 1; while(sl > -(long long)n_back && in[sl - 1] != '\n') --sl;
+    long long e1 = end - 1; while(e1 < (long long)n && in[e1] != '\n') ++e1;
+    long long e2 = e1 + 1;  while(e2 < (long long)n && in[e2] != '\n') ++e2;
+    if(e2 < (long long)n) qoff = e2 + 1 - sl;
+  }
   int got = 0;
   for(long long p = end - 1; got < need; --p) {
     if(p < 0) {
@@ -302,7 +313,8 @@ __device__ void backfill_fastq(const uint8_t* in, uint64_t n, const Carry* cin, 
     const uint32_t b = in[p];
     if(b == '\n') return;
     uint32_t sy;
-    if(b == '\r') { if(cr_dropped(in, (uint64_t)p, n)) continue; sy = SYM_BREAK; }
+    if(min_qual) sy = (qoff < 0 || p + qoff >= (long long)n || (signed char)in[p + qoff] < (signed char)min_qual) ? (uint32_t)SYM_BREAK : base_symbol(b);
+    else if(b == '\r') { if(cr_dropped(in, (uint64_t)p, n)) continue; sy = SYM_BREAK; }
     else sy = base_symbol(b);
     if(sy == SYM_BREAK) return;
     out[need - 1 - got] = (uint8_t)sy; ++got;
