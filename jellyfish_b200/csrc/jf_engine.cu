@@ -1750,10 +1750,12 @@ static int bam_header_field(jfgpu_engine* e, const char* p) {
   return JFGPU_OK;
 }
 
-// bytes of a record whose block_size field is at p
-static int bam_record_len(jfgpu_engine* e, const char* p, size_t cap, size_t* len) {
+// bytes of the record at byte `at` of the file, whose block_size field is at p
+static int bam_record_len(jfgpu_engine* e, const char* p, size_t cap, uint64_t at, size_t* len) {
   *len = 4 + (size_t)le32(p);
-  if(*len < 36) return fail(e, JFGPU_ERR_FORMAT, "Invalid BAM record: block_size " + std::to_string(*len - 4) + " is below the 32 bytes of its fixed fields");
+  if(*len < 36)
+    return fail(e, JFGPU_ERR_FORMAT, "Invalid BAM record at byte " + std::to_string(at) + " of the inflated file: block_size " +
+                std::to_string(*len - 4) + " is below the 32 bytes of its fixed fields");
   return *len > cap ? sam_too_long(e) : JFGPU_OK;
 }
 
@@ -1777,7 +1779,7 @@ static int bam_feed_host(jfgpu_engine* e, const char* bytes, size_t n, bool end)
       s.tail.append(bytes + pos, t); pos += t;
       if(s.tail.size() < head) break;
       size_t len = head;
-      if(s.bam_phase == BAM_RECORDS && (rc = bam_record_len(e, s.tail.data(), cap, &len))) return rc;
+      if(s.bam_phase == BAM_RECORDS && (rc = bam_record_len(e, s.tail.data(), cap, s.done_off, &len))) return rc;
       t = std::min(n - pos, len - s.tail.size());
       s.tail.append(bytes + pos, t); pos += t;
       if(s.tail.size() < len) break;
@@ -1798,8 +1800,11 @@ static int bam_feed_host(jfgpu_engine* e, const char* bytes, size_t n, bool end)
     size_t run = pos;
     uint32_t nr = 0;
     while(n - pos >= 4) {
-      size_t len = 0;
-      if((rc = bam_record_len(e, bytes + pos, cap, &len))) return rc;
+      size_t len = 4 + (size_t)le32(bytes + pos);
+      if(len < 36 || len > cap) {           // the records in front of it come first: a bad one among them is the first error
+        if(nr && (rc = sam_stage(e, bytes + run, pos - run, false, nr))) return rc;
+        return bam_record_len(e, bytes + pos, cap, s.done_off, &len);
+      }
       if(n - pos < len) break;
       if(pos + len - run > cap) {
         if((rc = sam_stage(e, bytes + run, pos - run, false, nr))) return rc;
@@ -1813,7 +1818,8 @@ static int bam_feed_host(jfgpu_engine* e, const char* bytes, size_t n, bool end)
     break;
   }
   if(end && (s.bam_phase != BAM_RECORDS || s.bam_skip || !s.tail.empty()))
-    return fail(e, JFGPU_ERR_FORMAT, s.bam_phase != BAM_RECORDS ? "Truncated BAM header" : "Truncated BAM record");
+    return fail(e, JFGPU_ERR_FORMAT, s.bam_phase != BAM_RECORDS || s.bam_skip ? std::string("Truncated BAM header")
+                                     : "Truncated BAM record at byte " + std::to_string(s.done_off) + " of the inflated file");
   return JFGPU_OK;
 }
 

@@ -143,8 +143,10 @@ __global__ void __launch_bounds__(1024) sam_tiles_kernel(uint32_t* tile_cnt, uin
     run += total;
   }
   if(threadIdx.x == 0) {
+    // More line starts than rec_cap: one of the first rec_cap - 1 lines is shorter than 11 bytes (rec_capacity), and (4) reports
+    // the first such line.  The error here only backstops that, at a position no line start reaches, so it never wins.
     res->n_recs = min(run, rec_cap);
-    if(run > rec_cap) set_error(res, 0, ERR_FIELDS);
+    if(run > rec_cap) set_error(res, hi - lo, ERR_FIELDS);
     const unsigned long long nl = res->last_nl;
     res->consumed = final ? hi - lo : nl ? nl - lo : 0;
   }

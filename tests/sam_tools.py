@@ -91,28 +91,45 @@ def bgzf(data, block=65280):
     return b"".join(bgzf_block(data[i:i + block]) for i in range(0, len(data), block)) + BGZF_EOF
 
 
-def sam_model_fastq(sam):
-    """The FASTQ `count --sam` counts for a SAM file: header ('@') and blank lines skipped, one '\\r' before a '\\n' dropped,
-    SEQ field 10 and QUAL field 11, a '*' SEQ gives no bases, a '*' QUAL gives every base the quality character 0x20, bytes
-    other than ACGTacgt become N.  Raises ValueError where the engine must refuse the file."""
+class FormatError(ValueError):
+    """Where the engine must refuse a file: `offset` is the byte of the file the engine's message names, `what` the reason
+    it gives."""
+
+    def __init__(self, offset, what):
+        super().__init__("%s (at byte %d)" % (what, offset))
+        self.offset, self.what = offset, what
+
+
+def sam_model_records(sam):
+    """[(byte offset of the line, its FASTQ record)] for the SAM lines that give bases; see sam_model_fastq."""
     out = []
     lines = sam.split(b"\n")
     last = lines.pop()                       # (b"" when the file ends with a newline)
     lines = [ln[:-1] if ln.endswith(b"\r") else ln for ln in lines] + ([last] if last else [])
-    for ln in lines:
+    at = 0
+    for ln, raw in zip(lines, sam.split(b"\n")):
+        start, at = at, at + len(raw) + 1
         if not ln or ln.startswith(b"@"):
             continue
         f = ln.split(b"\t")
         if len(f) < 11:
-            raise ValueError("fewer than 11 fields")
+            raise FormatError(start, "fewer than 11 fields")
         seq = b"" if f[9] == b"*" else f[9]
         if f[10] == b"*":
             qual = b" " * len(seq)
         elif len(f[10]) != len(seq):
-            raise ValueError("SEQ and QUAL of different lengths")
+            raise FormatError(start, "SEQ and QUAL of different lengths")
         else:
             qual = f[10]
         if seq:
             seq = bytes(c if c in b"ACGTacgt" else ord("N") for c in seq)
-            out.append(b"@\n" + seq + b"\n+\n" + qual + b"\n")
-    return b"".join(out)
+            out.append((start, b"@\n" + seq + b"\n+\n" + qual + b"\n"))
+    return out
+
+
+def sam_model_fastq(sam):
+    """The FASTQ `count --sam` counts for a SAM file: header ('@') and blank lines skipped, one '\\r' before a '\\n' dropped,
+    SEQ field 10 and QUAL field 11, a '*' SEQ gives no bases, a '*' QUAL gives every base the quality character 0x20, bytes
+    other than ACGTacgt become N.  Raises FormatError (a ValueError) with the offset of the first bad line where the engine
+    must refuse the file."""
+    return b"".join(r for _, r in sam_model_records(sam))
