@@ -652,7 +652,7 @@ static void resolve_win_events(jfgpu_engine* e, cudaStream_t st) {
 // k2_mode 3 and 4 take the window form too (include/jfgpu.h)
 static bool window_enabled(jfgpu_engine* e, const PartDev& pd) {
   return (e->p.k2_mode == 0 || e->p.k2_mode == 3 || e->p.k2_mode == 4) && e->op == 0 && e->tab.slot_bits == 32 && pd.rec_bytes == 4 &&
-         pd.region_bits > WIN_LG && pd.region_bits - WIN_LG <= 11 && CHUNK_BYTES == (WIN_ST_NTH / 2) * 16;
+         pd.region_bits > WIN_LG && pd.region_bits - WIN_LG <= 11;
 }
 // Whether a cleared table may stay zero in meaning only until its first drain: that drain takes the window form (plain
 // insertion, no Bloom prefilter) and then writes every slot of [0, local_size), and a deferred probe reaches less than one
@@ -696,7 +696,7 @@ int part_drain(jfgpu_engine* e, cudaStream_t st) {
   // window form: the first unit and the records of every region (chunk_scan_kernel, chunk_hist_kernel), on the host
   const uint32_t wpr_lg = win ? pd.region_bits - WIN_LG : 0;
   const uint64_t wpr = (uint64_t)1 << wpr_lg;
-  const size_t scatter_smem = ((size_t)4 * wpr + (size_t)WIN_ST_UNITS * pd.chunk_recs) * 4;
+  const size_t scatter_smem = win_scatter_smem(WIN_ST_UNITS, WIN_ST_NBUF, (uint32_t)wpr);
   std::vector<uint32_t> start(pd.P + 1);
   std::vector<unsigned long long> recs(pd.P);
   auto win_begin = [&]() -> int {
@@ -842,10 +842,10 @@ int part_drain(jfgpu_engine* e, cudaStream_t st) {
         if(stiles) {
           CUDA_OK(e, cudaMemsetAsync(ps.w_cursor.p, 0, ((size_t)G << wpr_lg) * 4, st));
           CUDA_OK(e, win_event(e, st));
-          win_scatter_kernel<true><<<stiles, WIN_ST_NTH, scatter_smem, st>>>(pd, wd, ps.order.as<uint32_t>(), hb); JF_LAUNCHED();
+          win_scatter_kernel<true><<<std::min<uint32_t>(stiles, e->n_sm), WIN_ST_NTH, scatter_smem, st>>>(pd, wd, ps.order.as<uint32_t>(), hb); JF_LAUNCHED();
           win_scan_kernel<<<1, 1024, 0, st>>>(wd, T0.stats); JF_LAUNCHED();
           CUDA_OK(e, win_event(e, st));
-          win_scatter_kernel<false><<<std::min<uint32_t>(stiles, e->n_sm * 2), WIN_ST_NTH, scatter_smem, st>>>(pd, wd, ps.order.as<uint32_t>(), hb);
+          win_scatter_kernel<false><<<std::min<uint32_t>(stiles, e->n_sm), WIN_ST_NTH, scatter_smem, st>>>(pd, wd, ps.order.as<uint32_t>(), hb);
           JF_LAUNCHED();
           CUDA_OK(e, win_event(e, st));
           if(e->kw == 1) {

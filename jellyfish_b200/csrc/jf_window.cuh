@@ -90,114 +90,183 @@ __global__ void __launch_bounds__(1024) win_scan_kernel(WinDev wd, unsigned long
 }
 
 // ---- tile sort by window, runs written to the group buffer ----------------------------------------
-// A tile = WIN_ST_UNITS chunks of one region (24 K records): histogram by window in shared memory, scan, stable placement in
-// a shared-memory staging buffer, then the runs (one per window, ~24 records) go to their places in the group buffer with
-// coalesced stores.  The GPU retires a bounded number of store transactions per second whatever their size
-// (scripts/micro/scatter_store.cu), so the tile is as large as two resident CTAs per SM allow.  The chunks are read twice
-// (second time from L2) instead of being held in registers across the scan.
-// BUCKETS (the bucket pass, one CTA per tile): the run of window gw goes to bucket gw after what earlier tiles put there;
-// a run that would overflow the bucket is not stored and flags the group.  Either way its length is added to wcursor[gw],
-// so the pass leaves every window's exact count behind.  Once a CTA sees the flag it stores nothing: the group is placed
-// again by the exact pass (!BUCKETS), which returns at once when the flag is clear and otherwise strides over the tiles
-// with a persistent grid, storing every run at the start win_scan gave it.
-constexpr uint32_t WIN_ST_UNITS = 12;
+// A tile = WIN_ST_UNITS chunks of one region (24 K records).  A persistent grid, one CTA of WIN_ST_NTH threads per SM, strides
+// over the group's tiles.  WIN_ST_NBUF tiles sit in shared memory at a time: while the CTA sorts and stores one, the TMA
+// engine brings in the next (cp.async.bulk + mbarrier), so every record is read from HBM once.  Each thread holds its
+// records in registers, and with each record its rank inside its window, which the histogram's shared-memory atomicAdd
+// returns; after the scan the records go back into the same buffer, sorted by window, and the runs (one per window, ~48
+// records at configs[1]) go to their places in the group buffer with coalesced stores.  Three block barriers per tile:
+// histogram complete (the previous tile's buffer is free: the next load is issued), warp totals of the scan, placement
+// complete.  The global atomicAdd that gives a run its place is issued before the placement and used after it.
+// BUCKETS (the bucket pass): the run of window gw goes to bucket gw after what earlier tiles put there; a run that would
+// overflow the bucket is not stored and flags the group.  Either way its length is added to wcursor[gw], so the pass leaves
+// every window's exact count behind.  Once a CTA sees the flag it sorts and stores nothing more, but still counts: the
+// group is placed again by the exact pass (!BUCKETS), which returns at once when the flag is clear and otherwise stores
+// every run at the start win_scan gave it.
+constexpr uint32_t WIN_ST_UNITS = 12;              // chunks per tile: the longest runs two tile buffers leave room for
+constexpr uint32_t WIN_ST_NBUF = 2;                // tiles in shared memory
 constexpr uint32_t WIN_ST_NTH = 1024;
 
-template<bool BUCKETS>
-__device__ __forceinline__ void win_scatter_tile(const PartDev& pd, const WinDev& wd, const uint32_t* __restrict__ order, uint32_t hb, uint32_t tile) {
-  extern __shared__ __align__(16) uint32_t wsm[];
-  const uint32_t wpr = 1u << wd.wpr_lg;
-  uint32_t* cnt = wsm; uint32_t* lbase = cnt + wpr; uint32_t* lcur = lbase + wpr; uint32_t* gbase = lcur + wpr;
-  uint32_t* stage = gbase + wpr;                   // WIN_ST_UNITS * chunk_recs records
-  __shared__ uint32_t warp_tot[WIN_ST_NTH / 32];
-  __shared__ uint32_t s_chunk[WIN_ST_UNITS], s_n[WIN_ST_UNITS];
+// dynamic shared memory of win_scatter_kernel: the tile buffers, then cnt, lbase and gbase (one word per window of a region)
+__host__ __device__ constexpr size_t win_scatter_smem(uint32_t units, uint32_t nbuf, uint32_t wpr) {
+  return (size_t)nbuf * units * CHUNK_BYTES + (size_t)3 * wpr * 4;
+}
+static_assert(win_scatter_smem(WIN_ST_UNITS, WIN_ST_NBUF, WIN_MAX_WPR) + 1024 <= 227 * 1024, "one CTA per SM");
+
+// (a persistent CTA of NTH threads; UNITS, NBUF and NTH are parameters so that scripts/micro/win_scatter.cu can compare tile shapes)
+template<bool BUCKETS, uint32_t UNITS, uint32_t NBUF, uint32_t NTH>
+__device__ __forceinline__ void win_scatter_tiles(const PartDev& pd, const WinDev& wd, const uint32_t* __restrict__ order, uint32_t hb) {
+  constexpr uint32_t CR = CHUNK_BYTES / 4;         // records per chunk (the window form takes 4-byte records only)
+  constexpr uint32_t V = UNITS * (CHUNK_BYTES / 16) / NTH;     // 16-byte pieces of a tile per thread
+  constexpr uint32_t PER_MAX = NTH >= WIN_MAX_WPR ? 1 : NTH * 2 >= WIN_MAX_WPR ? 2 : 4;     // windows per thread in the scan
+  static_assert(UNITS * (CHUNK_BYTES / 16) % NTH == 0 && NTH % 32 == 0 && NTH * PER_MAX >= WIN_MAX_WPR && NBUF >= 2 && UNITS <= 32, "tile shape");
+  static_assert(UNITS * CR <= 65536, "ranks are packed two to a word");
+  extern __shared__ __align__(128) uint32_t wsm[];
+  __shared__ __align__(8) uint64_t full[NBUF];
+  __shared__ uint32_t s_n[NBUF][UNITS];            // records of each chunk of the tile in each buffer
+  __shared__ uint32_t warp_tot[NTH / 32];
   __shared__ uint32_t s_skip;
-  const uint32_t tid = threadIdx.x;
-  for(uint32_t i = tid; i < wpr; i += WIN_ST_NTH) cnt[i] = 0;
-  // which region this tile belongs to (tiles are numbered region by region)
-  uint32_t r = 0;
-  while(r + 1 < wd.G && wd.stile_first[r + 1] <= tile) ++r;
-  const uint32_t u0 = wd.unit_first[r] + (tile - wd.stile_first[r]) * WIN_ST_UNITS;
-  const uint32_t u1 = min(u0 + WIN_ST_UNITS, wd.unit_first[r + 1]);
-  if(tid < WIN_ST_UNITS) {
-    uint32_t c = 0, n = 0;
-    if(u0 + tid < u1) { c = __ldg(order + u0 + tid); n = __ldg(&pd.dir[c].y); }
-    s_chunk[tid] = c; s_n[tid] = n;
+  if(!BUCKETS && *wd.overflow == 0) return;
+  const uint32_t wpr = 1u << wd.wpr_lg, wmask = wpr - 1;
+  uint32_t per_lg = 0;                             // (NTH << per_lg >= wpr)
+  while((NTH << per_lg) < wpr) ++per_lg;
+  const uint32_t per = 1u << per_lg;
+  uint32_t* const cnt = wsm + NBUF * UNITS * CR;
+  uint32_t* const lbase = cnt + wpr;               // warp-local exclusive prefix of the window counts
+  uint32_t* const gbase = lbase + wpr;             // output position = this + index in the sorted tile
+  const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+  const uint32_t n_mine = blockIdx.x < wd.n_tiles ? (wd.n_tiles - 1 - blockIdx.x) / gridDim.x + 1 : 0;
+  auto region_of = [&](uint32_t tile) { uint32_t r = 0; while(r + 1 < wd.G && wd.stile_first[r + 1] <= tile) ++r; return r; };
+  // warp 0, lane j < UNITS: chunk j of this CTA's k-th tile (NO_CHUNK past the tile's end), and its records
+  auto chunk_of = [&](uint32_t k) -> uint32_t {
+    if(k >= n_mine || lane >= UNITS) return NO_CHUNK;
+    const uint32_t tile = blockIdx.x + k * gridDim.x, r = region_of(tile);
+    const uint32_t u = wd.unit_first[r] + (tile - wd.stile_first[r]) * UNITS + lane;
+    return u < wd.unit_first[r + 1] ? __ldg(order + u) : NO_CHUNK;
+  };
+  auto recs_of = [&](uint32_t c) -> uint32_t { return c != NO_CHUNK ? min(__ldg(&pd.dir[c].y), CR) : 0u; };
+  // warp 0: the TMA engine brings this CTA's k-th tile into buffer k % NBUF
+  auto issue = [&](uint32_t k, uint32_t c, uint32_t n) {
+    const uint32_t b = k % NBUF, bytes = ((n + 3u) & ~3u) * 4u;
+    uint32_t sum = bytes;
+#pragma unroll
+    for(int o = 16; o; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    if(lane < UNITS) s_n[b][lane] = n;
+    __syncwarp();
+    if(lane == 0) { fence_proxy_async(); mbar_expect_tx(&full[b], sum); }   // (s_n is released by this arrival)
+    __syncwarp();
+    if(bytes) tma_load_1d(wsm + (b * UNITS + lane) * CR, pd.pool + (size_t)c * CHUNK_BYTES, bytes, &full[b]);
+  };
+
+  if(tid == 0) {
+    for(uint32_t b = 0; b < NBUF; ++b) mbar_init(&full[b], 1);
+    fence_proxy_async();
+    s_skip = 0;
   }
+  for(uint32_t i = tid; i < wpr; i += NTH) cnt[i] = 0;
   __syncthreads();
-  const uint32_t half = tid >> 9, piece = tid & 511u;      // two chunks per trip, 512 x 16 bytes each
-  const uint32_t wmask = wpr - 1;
+  uint32_t pc = NO_CHUNK, pn = 0;                  // warp 0: the next tile to issue (k + NBUF - 1 at tile k)
+  if(warp == 0) {
+    for(uint32_t k = 0; k + 1 < NBUF && k < n_mine; ++k) { const uint32_t c = chunk_of(k); issue(k, c, recs_of(c)); }
+    pc = chunk_of(NBUF - 1); pn = recs_of(pc);
+  }
+  bool skip = false;                               // (BUCKETS) the group's flag was seen: count only
+
+  for(uint32_t k = 0; k < n_mine; ++k) {
+    const uint32_t b = k % NBUF;
+    uint32_t* const buf = wsm + b * UNITS * CR;
+    mbar_wait(&full[b], (k / NBUF) & 1u);
+    // histogram; the rank a record gets there is its place in its window's run
+    uint32_t rec[4 * V], rank[2 * V];
 #pragma unroll
-  for(uint32_t it = 0; it < WIN_ST_UNITS / 2; ++it) {
-    const uint32_t j = 2 * it + half, n = s_n[j];
-    if(piece * 4 < n) {
-      const uint4 v = __ldg(reinterpret_cast<const uint4*>(pd.pool + (size_t)s_chunk[j] * CHUNK_BYTES) + piece);
-      const uint32_t rec[4] = { v.x, v.y, v.z, v.w };
+    for(uint32_t v = 0; v < V; ++v) {
+      const uint32_t x = tid + v * NTH, j = x / (CR / 4), q0 = (x % (CR / 4)) * 4, n = s_n[b][j];
+      const uint4 r4 = reinterpret_cast<const uint4*>(buf)[x];
+      rec[4 * v] = r4.x; rec[4 * v + 1] = r4.y; rec[4 * v + 2] = r4.z; rec[4 * v + 3] = r4.w;
+      rank[2 * v] = rank[2 * v + 1] = 0;
 #pragma unroll
-      for(uint32_t q = 0; q < 4; ++q) if(piece * 4 + q < n) atomicAdd(&cnt[((rec[q] >> hb) >> WIN_LG) & wmask], 1u);
+      for(uint32_t q = 0; q < 4; ++q)
+        if(q0 + q < n) rank[2 * v + q / 2] |= atomicAdd(&cnt[((rec[4 * v + q] >> hb) >> WIN_LG) & wmask], 1u) << (16 * (q & 1));
     }
-  }
-  __syncthreads();
-  // exclusive scan of cnt[0 .. wpr): each thread owns `per` consecutive windows
-  const uint32_t per = (wpr + WIN_ST_NTH - 1) / WIN_ST_NTH;
-  const uint32_t b = tid * per;
-  uint32_t s = 0;
-  for(uint32_t i = b; i < min(b + per, wpr); ++i) s += cnt[i];
-  uint32_t incl = s;
+    __syncthreads();                               // (1) histogram complete, the previous tile's buffer stored
+    if(warp == 0 && k + NBUF - 1 < n_mine) { issue(k + NBUF - 1, pc, pn); pc = chunk_of(k + NBUF); }
+    // exclusive scan of cnt: thread tid owns windows [tid * per, tid * per + per)
+    const uint32_t i0 = tid << per_lg;
+    uint32_t c[PER_MAX], s = 0;
 #pragma unroll
-  for(int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o); if((tid & 31) >= (uint32_t)o) incl += v; }
-  if((tid & 31) == 31) warp_tot[tid >> 5] = incl;
-  __syncthreads();
-  uint32_t woff = 0, total = 0;
-  for(uint32_t w = 0; w < WIN_ST_NTH / 32; ++w) { const uint32_t x = warp_tot[w]; if(w < (tid >> 5)) woff += x; total += x; }
-  uint32_t run = woff + incl - s;
-  for(uint32_t i = b; i < min(b + per, wpr); ++i) {
-    const uint32_t c = cnt[i];
-    lbase[i] = run; lcur[i] = run;
-    uint32_t at = 0;
-    if(c) {
-      const uint32_t gw = (r << wd.wpr_lg) + i;
-      at = atomicAdd(&wd.wcursor[gw], c);
-      if(BUCKETS) {
-        if(at + c <= wd.cap) at += gw * wd.cap;
-        else { at = (uint32_t)wd.wrec_cap; *(volatile uint32_t*)wd.overflow = 1u; }    // (every store of the run is past wrec_cap)
+    for(uint32_t p = 0; p < PER_MAX; ++p) { c[p] = p < per && i0 < wpr ? cnt[i0 + p] : 0u; s += c[p]; }
+    uint32_t incl = s;
+#pragma unroll
+    for(int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o); if(lane >= (uint32_t)o) incl += v; }
+    if(lane == 31) warp_tot[warp] = incl;
+    if(i0 < wpr) {
+      uint32_t x = incl - s;
+#pragma unroll
+      for(uint32_t p = 0; p < PER_MAX; ++p) if(p < per) { lbase[i0 + p] = x; x += c[p]; cnt[i0 + p] = 0; }
+    }
+    __syncthreads();                               // (2) warp totals
+    const uint32_t wt = lane < NTH / 32 ? warp_tot[lane] : 0u;
+    uint32_t winc = wt;
+#pragma unroll
+    for(int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, winc, o); if(lane >= (uint32_t)o) winc += v; }
+    const uint32_t wexcl = winc - wt, total = __shfl_sync(0xffffffffu, winc, 31);
+    // the runs' places: in the bucket pass the atomics are in flight while the records are placed
+    const uint32_t run0 = __shfl_sync(0xffffffffu, wexcl, warp) + incl - s;
+    const uint32_t r = region_of(blockIdx.x + k * gridDim.x);
+    uint32_t at[PER_MAX];
+    auto claim = [&] {
+#pragma unroll
+      for(uint32_t p = 0; p < PER_MAX; ++p) at[p] = c[p] ? atomicAdd(&wd.wcursor[(r << wd.wpr_lg) + i0 + p], c[p]) : 0u;
+    };
+    if(BUCKETS) claim();
+    uint32_t flag = 0;
+    if(BUCKETS && tid == 0) flag = *(volatile uint32_t*)wd.overflow;
+    if(!skip) {
+#pragma unroll
+      for(uint32_t v = 0; v < V; ++v) {
+        const uint32_t x = tid + v * NTH, j = x / (CR / 4), q0 = (x % (CR / 4)) * 4, n = s_n[b][j];
+#pragma unroll
+        for(uint32_t q = 0; q < 4; ++q) {
+          const uint32_t w = ((rec[4 * v + q] >> hb) >> WIN_LG) & wmask;
+          const uint32_t off = __shfl_sync(0xffffffffu, wexcl, (w >> per_lg) >> 5);
+          if(q0 + q < n) buf[lbase[w] + off + ((rank[2 * v + q / 2] >> (16 * (q & 1))) & 0xFFFFu)] = rec[4 * v + q];
+        }
       }
     }
-    gbase[i] = at - run;                           // (output position = this + index in the staging buffer)
-    run += c;
-  }
-  if(BUCKETS && tid == 0) s_skip = *(volatile uint32_t*)wd.overflow;
-  __syncthreads();
-  if(BUCKETS && s_skip) return;
+    if(!BUCKETS) claim();                          // (the exact pass, run only for a flagged group: after the placement, which
+                                                   // leaves no register for the atomics in flight)
+    if(i0 < wpr) {
+      uint32_t run = run0;
 #pragma unroll
-  for(uint32_t it = 0; it < WIN_ST_UNITS / 2; ++it) {
-    const uint32_t j = 2 * it + half, n = s_n[j];
-    if(piece * 4 < n) {
-      const uint4 v = __ldcs(reinterpret_cast<const uint4*>(pd.pool + (size_t)s_chunk[j] * CHUNK_BYTES) + piece);   // (L2 hit: read a moment ago)
-      const uint32_t rec[4] = { v.x, v.y, v.z, v.w };
-#pragma unroll
-      for(uint32_t q = 0; q < 4; ++q) if(piece * 4 + q < n) stage[atomicAdd(&lcur[((rec[q] >> hb) >> WIN_LG) & wmask], 1u)] = rec[q];
+      for(uint32_t p = 0; p < PER_MAX; ++p) if(p < per) {
+        uint32_t a = at[p];
+        if(BUCKETS && c[p]) {
+          const uint32_t gw = (r << wd.wpr_lg) + i0 + p;
+          if(a + c[p] <= wd.cap) a += gw * wd.cap;
+          else { a = (uint32_t)wd.wrec_cap; *(volatile uint32_t*)wd.overflow = 1u; flag = 1; }   // (every store of the run is past wrec_cap)
+        }
+        gbase[i0 + p] = a - run;
+        run += c[p];
+      }
     }
-  }
-  __syncthreads();
-  for(uint32_t i = tid; i < total; i += WIN_ST_NTH) {
-    const uint32_t v = stage[i], w = ((v >> hb) >> WIN_LG) & wmask;
-    const uint32_t dst = gbase[w] + i;
-    if(dst < wd.wrec_cap) wd.wrec[dst] = v;
+    if(BUCKETS && flag) s_skip = 1;
+    fence_proxy_async();                           // the placement's writes, before the TMA engine refills this buffer
+    __syncthreads();                               // (3) placement and run starts complete
+    if(BUCKETS) skip = s_skip != 0;
+    if(!skip) {
+      for(uint32_t i = tid; i < total; i += NTH) {
+        const uint32_t v = buf[i], w = ((v >> hb) >> WIN_LG) & wmask;
+        const uint32_t dst = gbase[w] + i;
+        if(dst < wd.wrec_cap) wd.wrec[dst] = v;
+      }
+    }
+    if(warp == 0) pn = recs_of(pc);                // (its latency is hidden behind the next tile's histogram)
   }
 }
 
 template<bool BUCKETS>
-__global__ void __launch_bounds__(WIN_ST_NTH, 2) win_scatter_kernel(PartDev pd, WinDev wd, const uint32_t* __restrict__ order, uint32_t hb) {
-  if constexpr(BUCKETS) {
-    win_scatter_tile<true>(pd, wd, order, hb, blockIdx.x);
-  } else {
-    if(*wd.overflow == 0) return;
-    for(uint32_t t = blockIdx.x; t < wd.n_tiles; t += gridDim.x) {
-      win_scatter_tile<false>(pd, wd, order, hb, t);
-      __syncthreads();                             // (the next tile reuses the shared memory)
-    }
-  }
+__global__ void __launch_bounds__(WIN_ST_NTH, 1) win_scatter_kernel(PartDev pd, WinDev wd, const uint32_t* __restrict__ order, uint32_t hb) {
+  win_scatter_tiles<BUCKETS, WIN_ST_UNITS, WIN_ST_NBUF, WIN_ST_NTH>(pd, wd, order, hb);
 }
 
 // ---- persistent window insert: probe in shared memory, windows and records moved by the TMA engine -------------
