@@ -119,3 +119,42 @@ def test_second_drain_into_a_table_in_memory(bucket_inputs, mode):
         with _counter(geometry, mode) as hc:
             st = _check(hc, bucket_inputs[geometry, "BD"], feeds=[[fas[0]], [fas[1]]])
         assert (st["seconds_win_hist"] == 0.0) if mode == 0 else (st["seconds_win_hist"] > 0)
+
+
+@pytest.mark.parametrize("mode", [0, 4])
+def test_2048_windows_per_region(built, mode):
+    """2^33 slots at k=17 in 128 MB regions: 256 regions of 2^25 slots, 2048 windows each, the widest geometry
+    window_enabled takes (every thread of the bucket pass's scan owns two windows; win_scan sees 131 072 windows in a
+    group of 64 regions).  About 200 Mbp of synthetic text, counted after a clear() (a write-only drain), through buckets
+    (mode 0) and through buckets without slack and the exact placement (mode 4), against the sort-based model: statistics,
+    histogram, sampled lookups and the digest of the whole dump.  (The C restatement cannot hold 2^33 slots.)"""
+    import torch
+    import kmer_model as km
+    from jellyfish_b200 import HashCounter, _lib
+    from test_gpu_bench_exact import _check_dump, _check_step, _queries, _synth
+    need = 40e9
+    free = torch.cuda.mem_get_info(0)[0]
+    if free < need:
+        pytest.skip("2^33 slots of 4 bytes, a 4 GB record pool and the model need about %.0f GB free, %.1f GB are" % (need / 1e9, free / 1e9))
+    lib = _lib.load()
+    n_bases = 200_000_000
+    text = torch.empty(lib.jfgpu_synth_fasta_bytes(n_bases) + 256, dtype=torch.uint8, device="cuda")
+    try:
+        n_text = _synth(lib, text, n_bases, 0x5EED2048 + mode)
+        queries = _queries(text, K, n_bases)
+        model = km.count(text[:n_text], K, queries=queries)
+        torch.cuda.empty_cache()
+        with HashCounter(1 << 33, 7, k=K, canonical=True, region_mb=128, pool_bytes=4 << 30, k2_mode=mode) as hc:
+            info = hc.info()
+            assert (info["lsize"], info["slot_bits"], info["part_regions"], info["part_rec_bytes"]) == (33, 32, 256, 4), info
+            hc.clear()
+            hc.add_device_text(text.data_ptr(), n_text)
+            st = hc.done()
+            what = "2048 windows per region, k2_mode %d" % mode
+            _check_step(hc, st, text[:n_text], K, info, model, queries, what)
+            _check_dump(hc, text[:n_text], K, info, model, what + ", dump")
+            assert st["seconds_win_scatter"] > 0 and st["seconds_win_insert"] > 0
+            assert (st["seconds_win_hist"] > 0) == (mode == 4)
+    finally:
+        del text
+        torch.cuda.empty_cache()
