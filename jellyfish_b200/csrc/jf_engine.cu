@@ -1258,8 +1258,9 @@ int rebuild_table(jfgpu_engine* e, unsigned nl, const jfb::gf2_matrix& M, int ol
   if(rc) return rc;
   // distinct / reprobes statistics restart for the new table; STAT_INSERTED counts k-mer
   // occurrences and must not change
-  unsigned long long inserted_before = 0;
+  unsigned long long inserted_before = 0, failed_before = 0;
   CUDA_OK(e, cudaMemcpyAsync(&inserted_before, e->stats.as<unsigned long long>() + STAT_INSERTED, 8, cudaMemcpyDeviceToHost, e->cs));
+  CUDA_OK(e, cudaMemcpyAsync(&failed_before, e->stats.as<unsigned long long>() + STAT_FAILED, 8, cudaMemcpyDeviceToHost, e->cs));
   CUDA_OK(e, cudaStreamSynchronize(e->cs));
   CUDA_OK(e, cudaMemsetAsync(e->stats.as<unsigned long long>() + STAT_DISTINCT, 0, 8, e->cs));
   CUDA_OK(e, cudaMemsetAsync(e->stats.as<unsigned long long>() + STAT_REPROBES, 0, 8, e->cs));
@@ -1275,7 +1276,20 @@ int rebuild_table(jfgpu_engine* e, unsigned nl, const jfb::gf2_matrix& M, int ol
     cudaStreamSynchronize(e->cs);
   }
   if(rc) return rc;
-  // the moved entries are not new k-mer occurrences; the failed ones (below) are
+  // the moved entries are not new k-mer occurrences; the failed ones (below) are.  A moved entry that found no slot in the
+  // new table (a clipped reprobe limit) waits in the failure list like a key that never reached a table, and is counted
+  // when the next table takes it: it leaves STAT_INSERTED now.
+  unsigned long long failed_after = 0;
+  CUDA_OK(e, cudaMemcpyAsync(&failed_after, e->stats.as<unsigned long long>() + STAT_FAILED, 8, cudaMemcpyDeviceToHost, e->cs));
+  CUDA_OK(e, cudaStreamSynchronize(e->cs));
+  failed_after = std::min<unsigned long long>(failed_after, e->fail_cap);
+  if(failed_after > failed_before) {
+    std::vector<uint64_t> waiting(failed_after - failed_before);
+    CUDA_OK(e, cudaMemcpyAsync(waiting.data(), e->fail_counts[e->fail_cur].as<uint64_t>() + failed_before, waiting.size() * 8,
+                               cudaMemcpyDeviceToHost, e->cs));
+    CUDA_OK(e, cudaStreamSynchronize(e->cs));
+    for(const uint64_t c : waiting) inserted_before -= c;
+  }
   CUDA_OK(e, cudaMemcpyAsync(e->stats.as<unsigned long long>() + STAT_INSERTED, &inserted_before, 8, cudaMemcpyHostToDevice, e->cs));
   CUDA_OK(e, cudaStreamSynchronize(e->cs));
   if(n_failed) {

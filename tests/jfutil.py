@@ -93,9 +93,9 @@ def key_words(keys, k):
 
 def positions(info, keys, k):
     """Original positions of Python int keys in a table described by HashCounter.info(), vectorised over the key words
-    (RectangularBinaryMatrix::times, as hash_pos)."""
+    (RectangularBinaryMatrix::times, as hash_pos).  keys may also be an (n, words) uint64 array, as text_model gives."""
     import numpy as np
-    words = key_words(keys, k)
+    words = keys if isinstance(keys, np.ndarray) else key_words(keys, k)
     size = info["size"]
     if info["matrix_identity"]:
         return words[:, 0] & np.uint64(size - 1)
