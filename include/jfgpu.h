@@ -208,6 +208,17 @@ int  jfgpu_seam_host(jfgpu_handle h, const char* bytes, size_t n, uint32_t flags
  * the caller zeroes).  Stream-ordered on `stream` (NULL = the engine's own stream); the caller synchronises before reading
  * the count.  Used to check that the shares of a FASTQ file start on record boundaries. */
 int  jfgpu_count_newlines(jfgpu_handle h, const void* dev_bytes, size_t n, uint64_t* dev_count, void* stream);
+/* Cut FASTQ text (device memory, 16-byte aligned) behind whole 4-line records, so that every piece can be handed to a feed
+ * of an engine with min_qual (-Q), which must end behind a record.  lines_mod4: the lines in front of dev_bytes (mod 4); a
+ * record ends behind a '\n' in front of which the number of lines is a multiple of 4.  The cuts c_1 < c_2 < ... go to
+ * `cuts` (host): c_i is the last record end at or before c_{i-1} + target (c_0 = 0), for as long as c_{i-1} + target < n.
+ * So every piece [c_{i-1}, c_i) and the last one [c_m, n) holds at most `target` bytes; *n_cuts = m (at most
+ * 2 * n / target + 1 when every record fits in target bytes).  *end_lines_mod4 (may be NULL): the lines (mod 4) at the end
+ * of the text.  A record that does not end within target bytes of the piece it starts is JFGPU_ERR_FORMAT, as a record
+ * larger than the staging batch of jfgpu_feed is; more than `cap` cuts is JFGPU_ERR_ARG.  Every byte is read once by one
+ * kernel, and one CTA resolves the cuts; the call synchronises `stream` once (NULL = the engine's own stream). */
+int  jfgpu_fastq_cuts(jfgpu_handle h, const void* dev_bytes, size_t n, uint32_t lines_mod4, uint64_t target, uint64_t* cuts,
+                      size_t cap, size_t* n_cuts, uint32_t* end_lines_mod4, void* stream);
 
 /* -- multi-GPU stages (no reference analogue; SURVEY.md section 8e) ------------------
  * Extract canonical k-mers from device-resident text and bucket them by owning shard

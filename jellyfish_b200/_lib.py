@@ -20,7 +20,7 @@ SYMBOLS = [
     "jfgpu_bloom_info_get", "jfgpu_bloom_load", "jfgpu_bloom_dump", "jfgpu_bloom_words", "jfgpu_bloom_fold", "jfgpu_bloom_dump_range",
     "jfgpu_set_spill", "jfgpu_shard_setup", "jfgpu_shard_round_bytes", "jfgpu_shard_extract", "jfgpu_shard_pack", "jfgpu_shard_unpack",
     "jfgpu_load_records", "jfgpu_query", "jfgpu_device_count", "jfgpu_seam", "jfgpu_seam_host", "jfgpu_count_newlines",
-    "jfgpu_sam_stage",
+    "jfgpu_sam_stage", "jfgpu_fastq_cuts",
 ]
 
 OK, ERR_ARG, ERR_CUDA, ERR_FULL, ERR_FORMAT, ERR_STATE, ERR_NOMEM, ERR_SINK = range(8)
@@ -170,6 +170,9 @@ def load():
     lib.jfgpu_seam_host.restype = C.c_int
     lib.jfgpu_count_newlines.argtypes = [H, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     lib.jfgpu_count_newlines.restype = C.c_int
+    lib.jfgpu_fastq_cuts.argtypes = [H, C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint64, C.POINTER(C.c_uint64), C.c_size_t,
+                                     C.POINTER(C.c_size_t), C.POINTER(C.c_uint32), C.c_void_p]
+    lib.jfgpu_fastq_cuts.restype = C.c_int
     lib.jfgpu_sam_stage.argtypes = [H, C.c_void_p, C.c_size_t, C.c_uint32, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_void_p]
     lib.jfgpu_sam_stage.restype = C.c_int
     lib.jfgpu_device_count.argtypes = []

@@ -238,6 +238,7 @@ struct jfgpu_engine {
   // jfgpu_seam: the ordered extraction runs into scratch that nobody reads (only the carry it leaves matters)
   bool seaming = false;
   DevBuf seam_keys, seam_cnt;
+  DevBuf fq_scratch;                        // jfgpu_fastq_cuts
   // SAM / BAM input (jf_sam.cu): the form of the file being fed (0 = FASTA / FASTQ text, 1 = SAM, 2 = BAM), the buffers of a
   // batch (made at the first such file; one of each: a batch is transcoded and read back before the next is staged) and what
   // a feed leaves to the next one
@@ -2138,6 +2139,30 @@ int jfgpu_count_newlines(jfgpu_handle e, const void* dev_bytes, size_t n, uint64
   cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
   g_launches.fetch_add(jfnl::count_newlines((const uint8_t*)dev_bytes, n, (unsigned long long*)dev_count, e->n_sm, st), std::memory_order_relaxed);
   CUDA_OK(e, cudaGetLastError());
+  return JFGPU_OK;
+}
+
+int jfgpu_fastq_cuts(jfgpu_handle e, const void* dev_bytes, size_t n, uint32_t lines_mod4, uint64_t target, uint64_t* cuts,
+                     size_t cap, size_t* n_cuts, uint32_t* end_lines_mod4, void* stream) {
+  if(!e || (n && !dev_bytes) || !n_cuts || (cap && !cuts) || target == 0) return JFGPU_ERR_ARG;
+  if(((uintptr_t)dev_bytes & 15) != 0) return fail(e, JFGPU_ERR_ARG, "device text must be 16-byte aligned");
+  cudaSetDevice(e->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
+  const size_t need_b = jfnl::fastq_cuts_scratch(n, cap);
+  if(e->fq_scratch.bytes < need_b && e->fq_scratch.alloc(need_b) != cudaSuccess)
+    return fail(e, JFGPU_ERR_NOMEM, "allocation of the FASTQ cut scratch failed");
+  g_launches.fetch_add(jfnl::fastq_cuts((const uint8_t*)dev_bytes, n, lines_mod4, target, cap, e->fq_scratch.p, st), std::memory_order_relaxed);
+  CUDA_OK(e, cudaGetLastError());
+  jfnl::FqResult r;
+  CUDA_OK(e, cudaMemcpyAsync(&r, e->fq_scratch.p, sizeof(r), cudaMemcpyDeviceToHost, st));
+  if(cap) CUDA_OK(e, cudaMemcpyAsync(cuts, (const uint8_t*)e->fq_scratch.p + sizeof(r), cap * 8, cudaMemcpyDeviceToHost, st));
+  CUDA_OK(e, cudaStreamSynchronize(st));
+  if(r.status == 1)
+    return fail(e, JFGPU_ERR_FORMAT, "Invalid fastq file: the record at byte " + std::to_string(r.fail_at) + " does not end within " +
+                std::to_string(target) + " bytes (a record larger than a piece, or one of more than 4 lines)");
+  if(r.status == 2) return fail(e, JFGPU_ERR_ARG, "jfgpu_fastq_cuts: more cuts than `cap`");
+  *n_cuts = (size_t)r.n_cuts;
+  if(end_lines_mod4) *end_lines_mod4 = (uint32_t)r.end_lines;
   return JFGPU_OK;
 }
 

@@ -95,6 +95,22 @@ def exchange_and_insert(backend, world, send, counts, capacity, recv, before_pay
 CHUNK = 8192          # bytes of a record chunk (jf_kernels.cuh CHUNK_BYTES)
 
 
+class _DeviceBytes(object):
+    """A byte range of device memory, seen by torch (CUDA array interface)."""
+
+    def __init__(self, ptr, n):
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": "|u1", "data": (ptr, False), "version": 2}
+
+
+def aligned_text(ptr, n, stage):
+    """ptr when it is 16-byte aligned (what the extraction takes), else the n bytes copied to the device tensor `stage` on
+    torch's current stream: a round of device text cut behind a FASTQ record starts anywhere."""
+    if ptr % 16 == 0 or n == 0:
+        return ptr
+    stage[:n].copy_(torch.as_tensor(_DeviceBytes(ptr, n), device=stage.device))
+    return stage.data_ptr()
+
+
 class RecordExchange(object):
     """The record form of the exchange (include/jfgpu.h, jfgpu_shard_*): every rank's K1 writes 4-byte records of the GLOBAL
     table's regions into a send pool whose chunk arenas belong to the owning shards; the chunks cross NVLink as they are
@@ -138,16 +154,20 @@ class RecordExchange(object):
         w, a = self.world, self.arena
         return [pool[((bank * w + d) * a) * unit:((bank * w + d) * a + counts[d]) * unit] for d in range(w)]
 
-    def add_device_text(self, ptr, n, begin, end):
-        self._rounds(n, begin, end, lambda off, ln, bank: ptr + off)
+    def add_device_text(self, ptr, n, begin, end, bounds=None):
+        """bounds: the piece bounds of the rounds ([0, ..., n], record_bounds); None: rounds of round_bytes."""
+        self._rounds(n, begin, end, lambda off, ln, bank: aligned_text(ptr + off, ln, self._stage_buf(bank)), bounds)
+
+    def _stage_buf(self, bank):
+        if getattr(self, "_stage", None) is None:
+            self._stage = [torch.empty(self.round_bytes + 256, dtype=torch.uint8, device=self.dev) for _ in range(2)]
+        return self._stage[bank]
 
     def _staged(self, hptr, ln, bank):
         """Copy ln bytes of pinned host text into the device staging buffer of `bank` on the extraction stream."""
         import ctypes as C
         from . import _lib
-        if getattr(self, "_stage", None) is None:
-            self._stage = [torch.empty(self.round_bytes + 256, dtype=torch.uint8, device=self.dev) for _ in range(2)]
-        dst = self._stage[bank].data_ptr()
+        dst = self._stage_buf(bank).data_ptr()
         if ln and _lib.load().jfgpu_memcpy_h2d(C.c_void_p(dst), C.c_void_p(hptr), ln, C.c_void_p(self.sa.cuda_stream)):
             raise RuntimeError("host to device copy failed")
         return dst
@@ -187,12 +207,14 @@ class RecordExchange(object):
         self._run(n_pieces, extract)
         return spent[0]
 
-    def _rounds(self, n, begin, end, fetch):
-        rounds = (n + self.round_bytes - 1) // self.round_bytes if n else 0
+    def _rounds(self, n, begin, end, fetch, bounds=None):
+        if bounds is None:
+            bounds = [min(n, r * self.round_bytes) for r in range((n + self.round_bytes - 1) // self.round_bytes + 1)] if n else [0]
+        rounds = len(bounds) - 1
 
         def extract(r, bank):
-            off = r * self.round_bytes
-            ln = max(0, min(self.round_bytes, n - off))
+            off = bounds[r] if r < rounds else n
+            ln = bounds[r + 1] - off if r < rounds else 0
             if ln or (r == 0 and begin) or (r == rounds_all[0] - 1 and end):
                 src = fetch(off, ln, bank)
                 self.hc.shard_extract(src, ln, bank, begin and r == 0, end and off + ln >= n, stream=self.sa.cuda_stream)
@@ -258,17 +280,26 @@ class ShareReader(object):
     of a trailing run of '\\r', which then begins the next piece: a device feed that ends on '\\r' takes the run for a line
     end, where the byte behind it decides.  A run of CR_SLACK bytes or more there is refused (ValueError).
 
+    records=True (FASTQ counted with -Q, whose feeds must end behind a whole record): a piece that is not the last one ends
+    instead behind the last complete 4-line record in front of its nominal end, found on the reading thread, and the next
+    piece starts there.  The nominal ends are then RECORD_SLACK (a quarter) of piece_bytes apart less, so that a piece is
+    never longer than piece_bytes; a record that does not end in that last quarter is refused (ValueError).  The pieces
+    still tile the share, so the newlines tallied over them are the share's.
+
     prefetch(i) reads piece i on a thread of its own, so that the disk or page-cache read overlaps the device work the
     caller enqueues meanwhile; read(i) then only waits for it."""
 
     CR_SLACK = 4096
+    RECORD_SLACK = 4        # records=True: the last piece_bytes // RECORD_SLACK bytes of a nominal piece hold its record end
 
-    def __init__(self, path, share, piece_bytes):
+    def __init__(self, path, share, piece_bytes, records=False):
         from . import _lib
         self._lib = _lib.load()
         self.fmt = share.fmt
         self.share = share
-        self.piece = max(1, piece_bytes - self.CR_SLACK)
+        self.records = records
+        self.slack = max(self.CR_SLACK, piece_bytes // self.RECORD_SLACK) if records else self.CR_SLACK
+        self.piece = max(1, piece_bytes - self.slack)
         n = max(0, share.end - share.start)
         self.n_pieces = (n + self.piece - 1) // self.piece
         self.fd = os.open(path, os.O_RDONLY)
@@ -288,7 +319,7 @@ class ShareReader(object):
         import ctypes as C
         b = i & 1
         if self.bufs[b] is None:
-            p = self._lib.jfgpu_host_alloc(self.piece + self.CR_SLACK)
+            p = self._lib.jfgpu_host_alloc(self.piece + self.slack)
             if not p:
                 raise MemoryError("pinned host allocation failed")
             self.bufs[b] = p
@@ -302,7 +333,9 @@ class ShareReader(object):
         if got != stop - off:
             raise IOError("short read of %d bytes at %d" % (stop - off, off))
         n = got
-        if not last:
+        if not last and self.records:
+            n = self._record_end(view, n, stop)
+        elif not last:
             tail = bytes(memoryview(view)[max(0, n - self.CR_SLACK):n])
             run = len(tail) - len(tail.rstrip(b"\r"))
             if run == len(tail):
@@ -311,6 +344,22 @@ class ShareReader(object):
             n -= run
         self.next_off = off + n
         return self.bufs[b], n, i == 0 and self.first_begins, last
+
+    def _record_end(self, view, n, stop):
+        """The length of the longest prefix of the n bytes read that ends behind a whole 4-line record (the piece starts on
+        one): the last '\n' of the last `slack` bytes whose index in the piece is a multiple of 4."""
+        import numpy as np
+        a = np.frombuffer(view, dtype=np.uint8, count=n)
+        step = 16 << 20
+        lines = sum(int(np.count_nonzero(a[o:o + step] == 10)) for o in range(0, n, step))
+        t0 = max(0, n - self.slack)
+        at = np.flatnonzero(a[t0:] == 10)
+        ends = at[(lines - len(at) + 1 + np.arange(len(at))) % 4 == 0]
+        if not len(ends):
+            raise ValueError("no FASTQ record ends in the %d bytes in front of byte %d, where the share is cut into pieces "
+                             "(a record of more than %d bytes, or records of more than 4 lines): count this file with "
+                             "--split files" % (n - t0, stop, self.slack))
+        return t0 + int(ends[-1]) + 1
 
     def prefetch(self, i):
         """Start reading piece i (the pieces before it have been read) on a thread; nothing when i is past the last."""
@@ -410,6 +459,8 @@ class ShardedCounter(object):
         if batch_bytes is None:
             batch_bytes = default_batch_bytes(k)
         self.rank, self.world = rank, world
+        # -Q: every feed of FASTQ text must end behind a whole record (include/jfgpu.h: jfgpu_params.min_qual)
+        self.qual = bool(engine_kw.get("min_qual"))
         self.hc = HashCounter(size, val_len, k=k, canonical=canonical, reprobes=reprobes, device=device,
                               shard_index=rank, n_shards=world, allow_regrow=(world == 1), max_batch_bytes=batch_bytes,
                               bf_size=bf_size, bf_fp=bf_fp, **engine_kw)
@@ -444,25 +495,44 @@ class ShardedCounter(object):
         # ops and NCCL collectives are ordered on one stream (handle 0 would mean "engine stream")
         self.stream = torch.cuda.Stream(device=self.dev)
 
-    def add_device_text(self, ptr, n, begin=True, end=True):
+    def add_device_text(self, ptr, n, begin=True, end=True, fastq=False):
+        """Device text, cut into exchange rounds.  fastq=True on an engine with -Q: the text is FASTQ that starts on a record
+        and, unless it ends the file, ends behind one; the rounds are then cut behind whole records (record_bounds)."""
         if self.world == 1:
             self.hc.add_device_text(ptr, n, begin=begin, end=end)
             return
         torch.cuda.current_stream(self.dev).synchronize()     # the caller's text is complete
+        budget = self.records.round_bytes if self.records is not None else self.batch_bytes
+        bounds = self.record_bounds(ptr, n, budget) if fastq and self.qual else None
         if self.records is not None:
-            self.records.add_device_text(ptr, n, begin, end)
+            self.records.add_device_text(ptr, n, begin, end, bounds)
             return
         with torch.cuda.stream(self.stream):
-            self._add_device_text(ptr, n, begin, end)
+            self._add_device_text(ptr, n, begin, end, bounds)
         self.stream.synchronize()
 
-    def _add_device_text(self, ptr, n, begin, end):
+    def record_bounds(self, ptr, n, budget):
+        """[0, c_1, ..., c_m, n]: FASTQ text in device memory cut behind whole records into pieces of at most `budget` bytes
+        (jfgpu_fastq_cuts: one pass over the text, one synchronisation)."""
+        if not n:
+            return [0]
+        cuts, _ = self.hc.fastq_cuts(ptr, n, budget)
+        return [0] + cuts + [n]
+
+    def _add_device_text(self, ptr, n, begin, end, bounds=None):
+        if bounds is None:
+            bounds = [min(n, i * self.batch_bytes) for i in range((n + self.batch_bytes - 1) // self.batch_bytes + 1)] if n else [0]
+
         def extract(i, send, counts):
-            off = i * self.batch_bytes
-            ln = max(0, min(self.batch_bytes, n - off))
+            if i + 1 >= len(bounds):              # (another rank has more rounds)
+                return
+            off, ln = bounds[i], bounds[i + 1] - bounds[i]
             if ln:
-                self.backend.extract_route((ptr + off, ln), begin and off == 0, end and off + ln >= n, send, self.capacity, counts)
-        self._pipeline((n + self.batch_bytes - 1) // self.batch_bytes, extract)
+                if (ptr + off) % 16 and self._piece_stage is None:
+                    self._piece_stage = [torch.empty(self.batch_bytes + 256, dtype=torch.uint8, device=self.dev) for _ in range(2)]
+                src = aligned_text(ptr + off, ln, self._piece_stage[i & 1] if self._piece_stage else None)
+                self.backend.extract_route((src, ln), begin and off == 0, end and off + ln >= n, send, self.capacity, counts)
+        self._pipeline(len(bounds) - 1, extract)
 
     def _pipeline(self, rounds, extract):
         """Two-stage software pipeline: the extraction of batch i+1 (stream A) overlaps the NVLink
@@ -641,6 +711,13 @@ class ShardedCounter(object):
             self._pipeline(reader.n_pieces, extract)
         self.stream.synchronize()
         return ok[0]
+
+    def set_op(self, op):
+        """COUNT, PRIME or UPDATE on this rank (HashCounter.set_op: what is staged is drained under the operation before).
+        Every rank switches at the same point of the exchange rounds: each add_* call returns once this rank has inserted,
+        or restaged into its own record pool, everything it received, and a peer's records of the next operation only
+        arrive through the next exchange round, which this rank enters after the switch."""
+        self.hc.set_op(op)
 
     def done(self):
         return self.hc.done()

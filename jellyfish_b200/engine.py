@@ -233,6 +233,17 @@ class HashCounter(object):
         """Add the '\\n' bytes of device text to the device uint64 at count_ptr (stream-ordered: jfgpu_count_newlines)."""
         self._check(self._lib.jfgpu_count_newlines(self._h, C.c_void_p(dev_ptr), n, C.c_void_p(count_ptr), C.c_void_p(stream or 0)))
 
+    def fastq_cuts(self, dev_ptr, n, target, lines_mod4=0, stream=None):
+        """Cut FASTQ text in device memory behind whole records into pieces of at most `target` bytes (include/jfgpu.h:
+        jfgpu_fastq_cuts).  lines_mod4: the lines in front of the text (mod 4).  -> (the cuts, lines (mod 4) at the end); the
+        pieces are [0, c_1), [c_1, c_2), ..., [c_m, n)."""
+        cap = 2 * (n // target) + 2
+        cuts = (C.c_uint64 * cap)()
+        got, end = C.c_size_t(0), C.c_uint32(0)
+        self._check(self._lib.jfgpu_fastq_cuts(self._h, C.c_void_p(dev_ptr), n, lines_mod4, target, cuts, cap, C.byref(got),
+                                               C.byref(end), C.c_void_p(stream or 0)))
+        return list(cuts[:got.value]), end.value
+
     def extract_route(self, dev_ptr, n, keys_ptr, capacity, counts_ptr, begin=True, end=True, stream=None, fmt=None):
         flags = text_flags(begin, end, fmt)
         self._check(self._lib.jfgpu_extract_route(self._h, C.c_void_p(dev_ptr), n, flags, C.c_void_p(keys_ptr),

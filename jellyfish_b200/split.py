@@ -12,6 +12,12 @@ non-base byte is a reset, which only shortens what must be carried; so parsing [
 symbols a parse of the whole file carries into s_r.  A share that starts on a header line needs no seam.  The seam is
 read whole: for FASTA whose sequences are not wrapped it is the whole sequence line in front of the cut.
 
+Under -Q (`headers=True`) a FASTA share starts on a header line instead: s_r is the first line start >= a_r whose first
+byte is '>'.  The parser with -Q reads '\r' by other rules than the seam knows (include/jfgpu.h, jfgpu_seam), and a share
+that starts on a header needs no seam.  A file of fewer records than ranks, or one whose records are few and long (a
+genome of a few chromosomes), then leaves some ranks an empty or a short share: the count is the same, only fewer GPUs
+parse it.
+
 FASTQ (4-line records): s_r is the first line start >= a_r where two consecutive records look whole ('@' line, a line,
 '+' line, a line as long as the sequence line).  Every read starts with a reset, so there is no seam.  This local rule is
 not exact -- a sequence line may start with '@' and a quality line with '+' -- so the caller checks every cut afterwards:
@@ -98,6 +104,22 @@ def fasta_seam_start(read, start, k):
     return c
 
 
+def fasta_header_at_or_after(read, size, a):
+    """The first line start >= a whose first byte is '>' (size when there is none)."""
+    if a <= 0:
+        return 0
+    p = a - 1                 # a header at q needs a '\n' at q - 1
+    while p < size:
+        w = read(p, min(WINDOW, size - p))
+        i = w.find(b"\n>")
+        if i >= 0:
+            return p + i + 1
+        if p + len(w) >= size:
+            break
+        p += len(w) - 1       # (the windows overlap by one byte: a "\n>" across two is found)
+    return size
+
+
 def _lines_from(read, size, p, n):
     """Up to n lines starting at the line start p -> list of (start, bytes without the '\\n')."""
     w = WINDOW
@@ -139,23 +161,26 @@ def fastq_share_start(read, size, a):
     return size
 
 
-def share_start(read, size, fmt, a):
-    """s for the nominal cut a (0 -> 0)."""
+def share_start(read, size, fmt, a, headers=False):
+    """s for the nominal cut a (0 -> 0).  headers: FASTA shares start on header lines (-Q)."""
     if a <= 0:
         return 0
-    return _line_start_at_or_after(read, size, a) if fmt == "fasta" else fastq_share_start(read, size, a)
+    if fmt == "fasta":
+        return fasta_header_at_or_after(read, size, a) if headers else _line_start_at_or_after(read, size, a)
+    return fastq_share_start(read, size, a)
 
 
-def plan_share(read, size, fmt, rank, world, k):
-    """Share of `rank` in a file of `size` bytes read through read(offset, n) -> bytes."""
-    s = share_start(read, size, fmt, rank * size // world)
-    e = size if rank == world - 1 else share_start(read, size, fmt, (rank + 1) * size // world)
+def plan_share(read, size, fmt, rank, world, k, headers=False):
+    """Share of `rank` in a file of `size` bytes read through read(offset, n) -> bytes.  headers=True (-Q): a FASTA share
+    starts on a header line and has no seam."""
+    s = share_start(read, size, fmt, rank * size // world, headers)
+    e = size if rank == world - 1 else share_start(read, size, fmt, (rank + 1) * size // world, headers)
     e = max(e, s)
-    seam = fasta_seam_start(read, s, k) if fmt == "fasta" and s < e else s
+    seam = fasta_seam_start(read, s, k) if fmt == "fasta" and s < e and not headers else s
     return Share(fmt, seam, s, e)
 
 
-def plan_file(path, rank, world, k):
+def plan_file(path, rank, world, k, headers=False):
     """plan_share of a regular file (pread; see `splittable`); None for an empty file.  ValueError: not FASTA or FASTQ
     text."""
     fd = os.open(path, os.O_RDONLY)
@@ -164,7 +189,7 @@ def plan_file(path, rank, world, k):
         fmt = sniff(os.pread(fd, 1, 0))
         if fmt is None:
             return None
-        return plan_share(lambda off, n: os.pread(fd, n, off), size, fmt, rank, world, k)
+        return plan_share(lambda off, n: os.pread(fd, n, off), size, fmt, rank, world, k, headers)
     finally:
         os.close(fd)
 
