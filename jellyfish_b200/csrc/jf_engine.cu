@@ -1436,6 +1436,17 @@ extern "C" {
 
 const char* jfgpu_version(void) { return "jellyfish-b200 0.1 (sm_90a)"; }
 uint64_t jfgpu_kernel_launches(void) { return g_launches.load(); }
+#if JF_K1_PROF
+// the instrumented build only (scripts/k1_phases.py): copy out the phase counters of the FAST K1 kernels of the current
+// device, then zero them
+int jfgpu_k1_prof(unsigned long long* out, int n) {
+  if(n != jfk::K1P_WORDS) return JFGPU_ERR_ARG;
+  static const unsigned long long zero[jfk::K1P_WORDS] = {};
+  if(cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(out, jfk::k1_prof_acc, sizeof(zero)) != cudaSuccess ||
+     cudaMemcpyToSymbol(jfk::k1_prof_acc, zero, sizeof(zero)) != cudaSuccess) return JFGPU_ERR_CUDA;
+  return JFGPU_OK;
+}
+#endif
 const char* jfgpu_last_error(jfgpu_handle h) { return h ? h->err.c_str() : g_create_error.c_str(); }
 
 void* jfgpu_host_alloc(size_t bytes) { void* p = nullptr; if(cudaHostAlloc(&p, bytes, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); return nullptr; } return p; }

@@ -20,7 +20,23 @@
 #define JF_EXTRACT_CUH
 #include "jf_kernels.cuh"
 
+// JF_K1_PROF=1 (only in the build scripts/k1_phases.py makes for itself): the FAST kernels stamp clock64() around each
+// block barrier and add, per warp, the cycles spent working in each segment and waiting at the barrier that ends it to
+// k1_prof_acc.  The product build leaves it at 0, and every kernel there compiles as if the stamps did not exist.
+#ifndef JF_K1_PROF
+#define JF_K1_PROF 0
+#endif
+
 namespace jfk {
+
+// segments of a window, each ended by a block barrier: TMA wait, B, C (scan), C (stream OR), D, E appends (4 per window),
+// ring passes (4 per window), E end, window end.  k1_prof_acc: work and wait cycles of every segment summed over warps, then
+// the hashing part of the E appends (per warp, no barrier), the warp-cycles of the window loop, windows, CTAs
+enum { K1P_TMA, K1P_B, K1P_C, K1P_OR, K1P_D, K1P_APPEND, K1P_PASS, K1P_EEND, K1P_WEND, K1P_SEGS };
+constexpr int K1P_WORDS = 2 * K1P_SEGS + 4;
+#if JF_K1_PROF
+static __device__ unsigned long long k1_prof_acc[K1P_WORDS];
+#endif
 
 // PREN = symbol positions kept in front of the window: PRE, or PRE_WIDE for four-word keys
 template<int NTH, int PREN = PRE>
@@ -147,6 +163,27 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t k = a.k;
   const uint64_t n = a.n;
+#if JF_K1_PROF
+  constexpr bool PROF = FAST;
+  __shared__ unsigned long long prof_w[NW][2 * K1P_SEGS + 2];   // per warp: work and wait cycles per segment, hashing, loop
+  long long prof_t = 0;                                          // when this warp left the last barrier
+  if(PROF && tid < NW * (2 * K1P_SEGS + 2)) (&prof_w[0][0])[tid] = 0;
+#endif
+  // a block barrier that ends segment s of a window (JF_K1_PROF: timed)
+  auto bsync = [&](const int s) {
+#if JF_K1_PROF
+    if constexpr(PROF) {
+      const long long t0 = clock64();
+      __syncthreads();
+      const long long t1 = clock64();
+      if(lane == 0) { prof_w[warp][2 * s] += t0 - prof_t; prof_w[warp][2 * s + 1] += t1 - t0; }
+      prof_t = t1;
+      return;
+    }
+#endif
+    (void)s;
+    __syncthreads();
+  };
 
   for(uint32_t i = tid; i < a.lut_bytes / 8; i += NTH) lut[i] = a.lut[i];
   if(a.bloom.mode) for(uint32_t i = tid; i < a.nbytes * 256; i += NTH) { bl1[i] = a.bloom.lut1[i]; bl2[i] = a.bloom.lut2[i]; }
@@ -176,26 +213,39 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
   }
   // FAST: one pass over the regions -- write the complete groups of 8 records of every ring to its chunk, close chunks that are
   // nearly full.  Between two barriers; `finish` also writes the incomplete group (end of the launch).
+  // Two threads per region: each group goes out as the two 16-byte halves of one 32-byte sector, written by neighbouring
+  // lanes in one store instruction, so it costs one store request instead of two; that took a third off the passes' time
+  // (DESIGN.md section 6, "K1 phase by phase").
   const uint32_t rlen = pd.ring_len;
-  // the word of slot s of region p's ring.  Every ring starts at bank 0 and a pass reads the rings of 32 consecutive regions
+  // the word of slot s of region p's ring.  Every ring starts at bank 0 and a pass reads the rings of consecutive regions
   // in 16-byte pieces at fill levels that are multiples of 8, which would touch only every other group of 4 banks: ring p is
   // rotated by 4 (p & 7) words so that they touch all of them
   auto ring_word = [&](const uint32_t p, const uint32_t s) -> uint32_t { return p * rlen + ((s + 4u * (p & 7u)) & (rlen - 1)); };
   auto flush_rings = [&](const bool finish) {
-    for(uint32_t p = tid; p < pd.P; p += NTH) {
-      const uint32_t v = st_cnt[p];
+    const uint32_t half = tid & 1u;                // which 16 bytes of a group this thread writes
+    // (every thread runs the same iterations, so the whole warp can meet at __syncwarp)
+    for(uint32_t base = 0; base < pd.P; base += NTH / 2) {
+      const uint32_t p = base + (tid >> 1);
+      const bool live = p < pd.P;
+      const uint32_t v = live ? st_cnt[p] : 0u;
       uint32_t cnt = v & 0xFFFFu, fl = v >> 16;
       const uint32_t lim = min(fl + rlen, pd.chunk_recs);
       if(cnt > lim) cnt = lim;                    // the slots beyond went to the spill list: hand them out again
-      const uint32_t c = st_chunk[p];
-      if(c == NO_CHUNK) continue;
+      const uint32_t c = live ? st_chunk[p] : NO_CHUNK;
       uint32_t* dst = reinterpret_cast<uint32_t*>(pd.pool + (size_t)c * CHUNK_BYTES);
-      while((fl & 7u) && fl < cnt) { dst[fl] = ring[ring_word(p, fl)]; ++fl; }          // (only after a launch that ended inside a group)
-      while(cnt - fl >= 8u) {
-        const uint4 x0 = *reinterpret_cast<const uint4*>(ring + ring_word(p, fl)), x1 = *reinterpret_cast<const uint4*>(ring + ring_word(p, fl + 4));
-        *reinterpret_cast<uint4*>(dst + fl) = x0; *reinterpret_cast<uint4*>(dst + fl + 4) = x1;
-        fl += 8;
+      if(c != NO_CHUNK) {
+        // (only after a launch that ended inside a group; both threads store the same words)
+        while((fl & 7u) && fl < cnt) { dst[fl] = ring[ring_word(p, fl)]; ++fl; }
+        while(cnt - fl >= 8u) {
+          const uint32_t s = fl + 4u * half;
+          *reinterpret_cast<uint4*>(dst + s) = *reinterpret_cast<const uint4*>(ring + ring_word(p, s));
+          fl += 8;
+        }
       }
+      // the rest of the region's pass is the first thread's: its writes of st_cnt[p] and st_chunk[p] wait until the second
+      // thread has read them
+      __syncwarp();
+      if(half || c == NO_CHUNK) continue;
       const bool close = cnt + min(rlen, pd.margin) > pd.chunk_recs;
       if(close || finish) for(; fl < cnt; ++fl) dst[fl] = ring[ring_word(p, fl)];
       if(close) {
@@ -212,6 +262,10 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
   for(uint32_t i = tid; i < NTH + PW + 2; i += NTH) sm.brk[i] = 0;
   if(tid == 0) mbar_init(&sm.bar, 1);
   __syncthreads();
+#if JF_K1_PROF
+  const long long prof_start = clock64();
+  prof_t = prof_start;
+#endif
 
   auto issue = [&](uint64_t t) {       // TMA copy of window t (thread 0 only)
     long long h = (long long)(t * (uint64_t)TILEB) - HALO;
@@ -247,7 +301,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
     }
     mbar_wait(&sm.bar, phase);
     phase ^= 1;
-    __syncthreads();
+    bsync(K1P_TMA);
 
     // ---- phase B: 32 bytes per thread, word-parallel classification ----
     uint32_t w[8];
@@ -317,7 +371,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
       if(lane >= o) inc = fn_compose(up, inc);
     }
     if(lane == 31) sm.warp_fn[warp] = inc;
-    __syncthreads();
+    bsync(K1P_B);
     uint32_t entry = (t == 0) ? (a.format == 1 ? (a.carry_in->state & 3u) : a.carry_in->state) : (uint32_t)a.tile_state[t];
     uint32_t wpre;
     {   // composition of the functions of the warps in front of this one: every warp scans the NW partials itself
@@ -426,7 +480,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
     }
     if(lane == 31) sm.warp_cnt[warp] = cinc;
     if(tid == 0) sm.halo_break = 0;
-    __syncthreads();
+    bsync(K1P_C);
     uint32_t woff;
     {
       uint32_t g = lane < NW ? sm.warp_cnt[lane] : 0u;
@@ -459,7 +513,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
         if(y1) atomicOr(sm.brk + (pos >> 5) + 1, y1);
       }
     }
-    __syncthreads();
+    bsync(K1P_OR);
     // the window's bytes are dead from here on (the per-byte paths above read them from shared memory): fetch the next one
     { const uint64_t tn = t + gridDim.x; if(tn < a.n_tiles && tid == 0) issue(tn); }
     const uint32_t idx0 = sm.idx0, nsym = sm.nsym;
@@ -492,7 +546,7 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
         sm.brk[q] = x;
       }
     }
-    __syncthreads();
+    bsync(K1P_D);
 
     // hand the parser state to the next batch
     if(t == a.n_tiles - 1 && warp == 1) {
@@ -722,6 +776,9 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
               // two passes over the SG k-mers so that the shared-memory round trips overlap: keys, hashes and records (4 SG
               // independent table loads in flight), then the slot reservations and the ring stores
               uint32_t P[SG], R[SG];
+#if JF_K1_PROF
+              const long long prof_h = clock64();
+#endif
 #pragma unroll
               for(int jj = 0; jj < SG; ++jj) {
                 const int j = hf + jj;
@@ -737,6 +794,9 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
                 P[jj] = (h32 >> f_rgb) | (ext << (32 - f_rgb));                       // region
                 R[jj] = ((h32 & f_relmask) << f_hb) | (uint32_t)(key[0] >> f_lsz);    // (position in the region, explicit key bits)
               }
+#if JF_K1_PROF
+              if(lane == 0) prof_w[warp][2 * K1P_SEGS] += clock64() - prof_h;
+#endif
 #pragma unroll
               for(int jj = 0; jj < SG; ++jj) if((vm4 >> jj) & 1u) ring_append(P[jj], R[jj], hf + jj);
             }
@@ -744,9 +804,9 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
             // top of at most 7 of an incomplete group and overflows in about 1e-6 of the region-passes, into the exact spill list.
             // The sharded send side cannot spill another shard's k-mer, so it keeps a pass per SG k-mers.
             if(hf + SG < 8 && !pd.by_owner) continue;
-            __syncthreads();
+            bsync(K1P_APPEND);
             flush_rings(false);
-            __syncthreads();
+            bsync(K1P_PASS);
           }
         } else {
 #pragma unroll
@@ -802,13 +862,25 @@ __global__ void __launch_bounds__(NTH, (NTH == 512 ? 2 : 1)) extract_kernel(cons
       }
     }
     }
-    __syncthreads();     // all reads of the streams done
+    bsync(K1P_EEND);     // all reads of the streams done
     // clear the stream words this window used (the next window ORs into them) and roll full chunks over
     for(uint32_t i = tid; i < 2 * (n_words + PW) + 3; i += NTH) sm.rev[i] = 0;
     for(uint32_t i = tid; i < n_words + PW + 2; i += NTH) sm.brk[i] = 0;
     if(MODE == 2 && !FAST) for(uint32_t p = tid; p < pd.P; p += NTH) roll_chunk(pd, p, a.T.stats, st_chunk, st_cnt);
-    __syncthreads();
+    bsync(K1P_WEND);
   }
+#if JF_K1_PROF
+  if constexpr(PROF) {
+    if(lane == 0) {
+      prof_w[warp][2 * K1P_SEGS + 1] = clock64() - prof_start;
+      for(int i = 0; i < 2 * K1P_SEGS + 2; ++i) atomicAdd(&k1_prof_acc[i], prof_w[warp][i]);
+    }
+    if(tid == 0) {
+      atomicAdd(&k1_prof_acc[2 * K1P_SEGS + 2], (unsigned long long)(blockIdx.x < a.n_tiles ? (a.n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0));
+      atomicAdd(&k1_prof_acc[2 * K1P_SEGS + 3], 1ull);
+    }
+  }
+#endif
   if(MODE == 2) {          // keep the open chunks for the next launch
     if(FAST) { flush_rings(true); __syncthreads(); }
     for(uint32_t p = tid; p < pd.P; p += NTH) { my_chunk[p] = st_chunk[p]; my_fill[p] = min(FAST ? (st_cnt[p] & 0xFFFFu) : st_cnt[p], pd.chunk_recs); }
