@@ -43,8 +43,18 @@ error of the rank that reads it: with two or more ranks the others then wait for
 Bloom structures (k <= 64) take the key exchange: `--bc FILE` is loaded whole by every rank and tested before a k-mer is
 routed; `--bf-size N` (the GLOBAL expected number of k-mers) gives every rank a filter for its share, applied by the
 owner after the exchange, where every occurrence of a k-mer arrives.
+
+`--disk`: a shard never doubles; when this rank's shard is full it is written to `OUT.<rank>.<i>` (i = 0, 1, ...), zeroed,
+and counting goes on, with no wait for the other ranks.  At the end a rank that never spilled writes `OUT.<rank>` with
+-L/-U as usual; a rank that spilled writes its table as one more piece, merges its pieces into `OUT.<rank>` (the `merge`
+of the command-line driver, -L/-U applied to the sums) and deletes them unless `--no-unlink` is given; rank 0
+concatenates.  The result is the single-GPU `count --disk` output for any world size.  `--no-merge` (once some rank has
+spilled) leaves every rank's pieces and writes no OUT: `jellyfish merge -o OUT OUT.*.*` gives it.  When a cut check fails
+every rank deletes its pieces before the files are counted again.  `--disk --if` is refused.  Without `--disk`,
+`--no-merge` and `--no-unlink` do nothing.
 """
 import argparse
+import datetime
 import os
 import sys
 import time
@@ -66,6 +76,10 @@ def _size(v):
 # An error found by one rank alone (a FASTQ record too long for a piece or a round under -Q, a run of '\r' where a share is
 # cut) ends that rank; the others are then left in the next collective until the job launcher's timeout ends them.
 _PEERS_WAIT = " (this rank stops here; the other ranks wait for it until the launcher's timeout)"
+
+# --disk: how long a rank waits in a collective for the others (NCCL's default is 10 minutes), long enough for a peer that
+# writes a full shard or merges its pieces on the CPU
+DISK_TIMEOUT_S = 6 * 3600
 
 
 def _count_whole(sc, path, owner):
@@ -208,6 +222,10 @@ def parse_args(argv=None):
     ap.add_argument("--quality-start", type=int, default=64, help="the quality character of --min-quality 0")
     ap.add_argument("--if", dest="if_files", action="append", default=[], metavar="PATH",
                     help="count only the k-mers of this file (may be given several times)")
+    ap.add_argument("--disk", action="store_true",
+                    help="a full shard is written to OUT.<rank>.<i>, zeroed, and counting goes on; the pieces are merged at the end")
+    ap.add_argument("--no-merge", action="store_true", help="--disk: leave the pieces OUT.<rank>.<i> and write no OUT")
+    ap.add_argument("--no-unlink", action="store_true", help="--disk: keep the pieces after merging them")
     ap.add_argument("files", nargs="*")
     a = ap.parse_args(argv)
 
@@ -236,6 +254,9 @@ def parse_args(argv=None):
     if a.mer_len > 64 and (a.bf_size or a.bc):
         sys.stderr.write("Error: --bf-size and --bc take mer lengths up to 64\n")
         sys.exit(1)
+    if a.disk and a.if_files:
+        # which primed keys a spill keeps depends on when each shard fills: no count of the reference's to be held to
+        error("--disk with --if is not supported on several GPUs (the keys primed before a spill would be lost)")
     return a
 
 
@@ -247,7 +268,9 @@ def main(argv=None):
     if world > 1:
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         os.environ.setdefault("NCCL_MAX_CTAS", "16")      # K1 leaves 16 SMs to the exchange that runs beside it
-        dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+        # --disk: a rank that spills or merges keeps the others waiting in the next collective or the final barrier
+        timeout = {"timeout": datetime.timedelta(seconds=DISK_TIMEOUT_S)} if a.disk else {}
+        dist.init_process_group("nccl", device_id=torch.device("cuda", local), **timeout)
     run(a, argv, rank, world, local)
 
 
@@ -274,7 +297,8 @@ def _prime(sc, a, count):
 
 def _count(a, argv, rank, world, local):
     sc = ShardedCounter(a.size, a.counter_len, k=a.mer_len, canonical=a.canonical, rank=rank, world=world, device=local,
-                        reprobes=a.reprobes, bf_size=a.bf_size, bf_fp=a.bf_fp, bc=a.bc, min_qual=a.min_qual)
+                        reprobes=a.reprobes, bf_size=a.bf_size, bf_fp=a.bf_fp, bc=a.bc, min_qual=a.min_qual,
+                        disk=a.output if a.disk else None, out_counter_len=a.out_counter_len)
     sc.sam_inflate_s = sc.sam_wall_s = 0.0
     if a.split == "files":
         _prime(sc, a, lambda files: count_files(sc, files, rank, world))
@@ -289,6 +313,8 @@ def _count(a, argv, rank, world, local):
                 what = "a FASTQ share does not start on a record" if not fastq_ok else \
                     "a SAM/BAM share could not be counted on its own (a BAM record chain does not meet the next share)"
                 sys.stderr.write("count_multi: %s; counting whole files per rank instead\n" % what)
+            if sc.disk:
+                sc.disk.discard_pieces()     # (no piece of the abandoned pass may reach the merge)
             sc.hc.clear()
             _prime(sc, a, lambda files: count_files(sc, files, rank, world))
             count_files(sc, a.files, rank, world)
@@ -299,10 +325,24 @@ def _count(a, argv, rank, world, local):
         sys.stderr.write("count_multi: rank %d --sam times: inflate_s %.4f transcode_route_s %.4f sam_wall_s %.4f\n"
                          % (rank, sc.sam_inflate_s, sc.sam_device_s, sc.sam_wall_s))
     cmdline = ["count_multi"] + (argv if argv is not None else sys.argv[1:])
-    sc.hc.dump("%s.%d" % (a.output, rank), lower=a.lower_count, upper=a.upper_count, out_counter_len=a.out_counter_len, cmdline=cmdline)
+    shard = "%s.%d" % (a.output, rank)
+    if not a.disk:
+        sc.hc.dump(shard, lower=a.lower_count, upper=a.upper_count, out_counter_len=a.out_counter_len, cmdline=cmdline)
+        pieces_only = False
+    else:
+        # --no-merge leaves pieces only once some rank has spilled: a count that never filled a shard writes OUT, as the
+        # single-GPU count --disk does
+        pieces_only = a.no_merge and not all_ranks_ok(not sc.disk.pieces, world, "cuda")
+        spills = len(sc.disk.pieces)
+        merge_s = sc.disk.write_output(shard, a.lower_count, a.upper_count, cmdline, merge=not pieces_only, unlink=not a.no_unlink)
+        # (read by scripts/disk_multi_bench.py)
+        sys.stderr.write("count_multi: rank %d --disk: spills %d spill_s %.4f merge_s %.4f\n" % (rank, spills, sc.disk.spill_s, merge_s))
     if world > 1:
         dist.barrier()
-    if rank == 0:
+    if pieces_only:
+        if rank == 0:
+            sys.stderr.write("count_multi: --no-merge: pieces %s.<rank>.<i> left for `jellyfish merge`\n" % a.output)
+    elif rank == 0:
         concat_shards(a.output, world, a.output)
         if not a.keep_shards:
             for r in range(world):

@@ -1344,7 +1344,7 @@ int regrow(jfgpu_engine* e) {
     if(e->h_stats[STAT_FAIL_DROPPED]) return fail(e, JFGPU_ERR_FULL, "Hash full (too many keys failed before the table could be doubled)");
     const unsigned kbits = 2 * e->k;
     if(!e->p.allow_regrow || e->shard_bits || (kbits < 64 && e->tab.size >= ((uint64_t)1 << kbits))) {
-      if(e->spill_fn && !e->shard_bits) { rc = spill_table(e, n_failed); if(rc) return rc; continue; }
+      if(e->spill_fn) { rc = spill_table(e, n_failed); if(rc) return rc; continue; }
       return fail(e, JFGPU_ERR_FULL, "Hash full");
     }
     const unsigned nl = e->tab.lsize + 1;
@@ -1425,6 +1425,16 @@ int check_after_batches(jfgpu_engine* e) {
     return regrow(e);
   }
   return JFGPU_OK;
+}
+
+// A spill hook is set on an engine that inserts on a caller's stream (jfgpu_insert_keys, jfgpu_shard_unpack): once the work
+// enqueued on `st` is done, keys that found no slot spill the table now, behind the drain of the pending region records, so
+// that the failure list holds at most what the next slice adds (one failure group) when the slice begins.
+int spill_if_failed(jfgpu_engine* e, cudaStream_t st) {
+  CUDA_OK(e, cudaStreamSynchronize(st));
+  CUDA_OK(e, cudaMemcpyAsync(e->h_stats + STAT_FAILED, e->stats.as<unsigned long long>() + STAT_FAILED, 8, cudaMemcpyDeviceToHost, e->cs));
+  CUDA_OK(e, cudaStreamSynchronize(e->cs));
+  return e->h_stats[STAT_FAILED] ? check_after_batches(e) : JFGPU_OK;
 }
 
 }  // namespace
@@ -2294,33 +2304,29 @@ int jfgpu_shard_pack(jfgpu_handle e, uint32_t bank, uint64_t* counts, void* stre
   return JFGPU_OK;
 }
 
-int jfgpu_shard_unpack(jfgpu_handle e, const uint64_t* counts, uint32_t self_bank, void* stream) {
-  if(!e || !counts) return JFGPU_ERR_ARG;
-  if(!e->sh.on) return fail(e, JFGPU_ERR_STATE, "jfgpu_shard_setup has not been called");
-  cudaSetDevice(e->device);
-  cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
+// restage_kernel over chunks [first, first + count[s]) of every source s's segment (one launch)
+static int restage_chunks(jfgpu_engine* e, const uint64_t* count, uint64_t first, uint32_t self_bank, cudaStream_t st) {
   const uint32_t G = e->p.n_shards;
   PartState& ps = e->part;
-  int rc = part_alloc(e);
-  if(rc) return rc;
   uint64_t total = 0;
-  for(uint32_t s = 0; s < G; ++s) { if(counts[s] > std::max(e->sh.seg_chunks, e->sh.arena_chunks)) return fail(e, JFGPU_ERR_ARG, "more chunks than a receive segment holds"); total += counts[s]; }
+  for(uint32_t s = 0; s < G; ++s) total += count[s];
   if(total == 0) return JFGPU_OK;
   // room in the CTAs' arenas of the local pool for the records of the received chunks (chunk j goes to CTA j mod grid)
   const uint64_t per_cta = (total + e->n_sm - 1) / e->n_sm + 1;
-  rc = part_reserve(e, st, chunks_for(ps, per_cta * (CHUNK_BYTES / 4)), "record pool smaller than one exchange round");
+  int rc = part_reserve(e, st, chunks_for(ps, per_cta * (CHUNK_BYTES / 4)), "record pool smaller than one exchange round");
   if(rc) return rc;
   rc = table_materialize(e, e->tab, st);      // (restage_kernel inserts the records of a full ring or chunk into the table itself)
   if(rc) return rc;
   RestageArgs ra;
   memset(&ra, 0, sizeof(ra));
   ra.T = table_dev(e, e->tab);
-  ra.recv_pool = e->sh.recv_pool; ra.recv_dir = e->sh.recv_dir; ra.n_src = G; ra.seg_chunks = (uint32_t)e->sh.seg_chunks;
-  for(uint32_t s = 0; s < G; ++s) ra.count[s] = (uint32_t)counts[s];
+  // (the kernel reads chunk rel of source s at s * seg_chunks + rel: the pools seen from chunk `first` on)
+  ra.recv_pool = e->sh.recv_pool + first * CHUNK_BYTES; ra.recv_dir = e->sh.recv_dir + first; ra.n_src = G; ra.seg_chunks = (uint32_t)e->sh.seg_chunks;
+  for(uint32_t s = 0; s < G; ++s) ra.count[s] = (uint32_t)count[s];
   ra.first_region = e->p.shard_index * e->sh.own_regions; ra.split_lg = e->sh.split_lg; ra.sbits = e->sh.sbits;
   ra.inv_lut = e->tab.inv_lut.as<uint64_t>(); ra.nbytes = e->nbytes;
   if(self_bank <= 1) {             // this shard's own chunks stay in its arena of that send bank
-    const size_t a0 = ((size_t)self_bank * G + e->p.shard_index) * e->sh.arena_chunks;
+    const size_t a0 = ((size_t)self_bank * G + e->p.shard_index) * e->sh.arena_chunks + first;
     ra.self_pool = e->sh.send_pool + a0 * CHUNK_BYTES; ra.self_dir = e->sh.send_dir + a0; ra.self_src = e->p.shard_index;
   }
   PartDev pd = part_dev(e);
@@ -2332,13 +2338,36 @@ int jfgpu_shard_unpack(jfgpu_handle e, const uint64_t* counts, uint32_t self_ban
   return JFGPU_OK;
 }
 
-int jfgpu_insert_keys(jfgpu_handle e, const void* dev_keys, uint64_t n, void* stream) {
-  if(!e) return JFGPU_ERR_ARG;
-  if(!e->tab.slots.p) return fail(e, JFGPU_ERR_STATE, "this engine holds a Bloom counter, not a hash table");
+int jfgpu_shard_unpack(jfgpu_handle e, const uint64_t* counts, uint32_t self_bank, void* stream) {
+  if(!e || !counts) return JFGPU_ERR_ARG;
+  if(!e->sh.on) return fail(e, JFGPU_ERR_STATE, "jfgpu_shard_setup has not been called");
   cudaSetDevice(e->device);
   cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
-  if(n == 0) return JFGPU_OK;
-  if(!stream) cudaEventRecord(e->ev_t0, st);
+  const uint32_t G = e->p.n_shards;
+  int rc = part_alloc(e);
+  if(rc) return rc;
+  uint64_t total = 0;
+  for(uint32_t s = 0; s < G; ++s) { if(counts[s] > std::max(e->sh.seg_chunks, e->sh.arena_chunks)) return fail(e, JFGPU_ERR_ARG, "more chunks than a receive segment holds"); total += counts[s]; }
+  const uint64_t slice = std::max<uint64_t>(1, e->fail_group / (CHUNK_BYTES / 4));      // chunks of at most one failure group
+  if(!e->spill_fn || total <= slice) {
+    rc = restage_chunks(e, counts, 0, self_bank, st);
+    return rc || !e->spill_fn ? rc : spill_if_failed(e, st);
+  }
+  // a spill hook and more records than one failure group (every one of them may meet a full ring or chunk): one source's
+  // chunks at a time, cut into slices
+  for(uint32_t s = 0; s < G; ++s)
+    for(uint64_t first = 0; first < counts[s]; first += slice) {
+      uint64_t one[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
+      one[s] = std::min(slice, counts[s] - first);
+      rc = restage_chunks(e, one, first, self_bank, st);
+      if(!rc) rc = spill_if_failed(e, st);
+      if(rc) return rc;
+    }
+  return JFGPU_OK;
+}
+
+// the keys of jfgpu_insert_keys into the table, or as region records into the pool, on `st`
+static int insert_key_slice(jfgpu_engine* e, const void* dev_keys, uint64_t n, cudaStream_t st) {
   int rc = JFGPU_OK;
   // --bf-size on a shard: the prefilter runs here, on the owner, where every occurrence of a key arrives (K1 routes them
   // unfiltered, run_batch).  Its matrices are the same draws as on every other shard, also when this one has routed nothing.
@@ -2397,6 +2426,24 @@ int jfgpu_insert_keys(jfgpu_handle e, const void* dev_keys, uint64_t n, void* st
     rc = insert_keys_into(e, e->tab, (const uint64_t*)dev_keys, nullptr, n, st);
     if(rc) return rc;
   }
+  return JFGPU_OK;
+}
+
+int jfgpu_insert_keys(jfgpu_handle e, const void* dev_keys, uint64_t n, void* stream) {
+  if(!e) return JFGPU_ERR_ARG;
+  if(!e->tab.slots.p) return fail(e, JFGPU_ERR_STATE, "this engine holds a Bloom counter, not a hash table");
+  cudaSetDevice(e->device);
+  cudaStream_t st = stream ? (cudaStream_t)stream : e->cs;
+  if(n == 0) return JFGPU_OK;
+  if(!stream) cudaEventRecord(e->ev_t0, st);
+  // with a spill hook, slices of at most one failure group, each followed by the spill its failed keys call for
+  const uint64_t slice = e->spill_fn ? e->fail_group : n;
+  for(uint64_t off = 0; off < n; off += slice) {
+    const uint64_t m = std::min(slice, n - off);
+    int rc = insert_key_slice(e, (const uint64_t*)dev_keys + off * e->kw, m, st);
+    if(!rc && e->spill_fn) rc = spill_if_failed(e, st);
+    if(rc) return rc;
+  }
   if(stream) return JFGPU_OK;          // stream-ordered: the caller synchronises
   cudaEventRecord(e->ev_t1, st);
   CUDA_OK(e, cudaStreamSynchronize(st));
@@ -2415,7 +2462,6 @@ int jfgpu_set_op(jfgpu_handle e, uint32_t op) {
 
 int jfgpu_set_spill(jfgpu_handle e, jfgpu_spill_fn fn, void* ctx) {
   if(!e) return JFGPU_ERR_ARG;
-  if(e->shard_bits) return fail(e, JFGPU_ERR_STATE, "spilling is not supported on a sharded table");
   e->spill_fn = fn; e->spill_ctx = ctx;
   return JFGPU_OK;
 }

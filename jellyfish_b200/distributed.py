@@ -19,6 +19,8 @@ import time
 import torch
 import torch.distributed as dist
 
+UINT64_MAX = (1 << 64) - 1
+
 
 class RouteBackend(object):
     """What the exchange needs from the engine; the CUDA engine implements it with kernels."""
@@ -449,10 +451,14 @@ class ShardedCounter(object):
     Bloom structures (k <= 64): `bf_size` (count --bf-size, the GLOBAL expected number of k-mers; `bf_fp` its false positive
     rate) puts a prefilter in front of every shard, applied by the owner after the exchange; `bc` (count --bc) is the path of
     a counter written by `jellyfish bc`, loaded whole by every rank and applied by the sender before the exchange.  Both take
-    the key exchange: the record exchange applies no filter."""
+    the key exchange: the record exchange applies no filter.
+
+    `disk` (count --disk) is a path prefix: the table does not double, and whenever this rank's shard is full it is written
+    to a piece with `out_counter_len` bytes a count, zeroed, and counting goes on (`self.disk`, DiskPieces)."""
 
     def __init__(self, size, val_len=7, k=None, canonical=False, rank=0, world=1, device=0, reprobes=126,
-                 batch_bytes=None, slack=1.25, exchange="auto", send_gb=None, bf_size=0, bf_fp=0.0, bc=None, **engine_kw):
+                 batch_bytes=None, slack=1.25, exchange="auto", send_gb=None, bf_size=0, bf_fp=0.0, bc=None, disk=None,
+                 out_counter_len=4, **engine_kw):
         from .engine import HashCounter
         if bf_size and bc:
             raise ValueError("Switches [--bf-size] and [--bc] conflict")
@@ -462,8 +468,9 @@ class ShardedCounter(object):
         # -Q: every feed of FASTQ text must end behind a whole record (include/jfgpu.h: jfgpu_params.min_qual)
         self.qual = bool(engine_kw.get("min_qual"))
         self.hc = HashCounter(size, val_len, k=k, canonical=canonical, reprobes=reprobes, device=device,
-                              shard_index=rank, n_shards=world, allow_regrow=(world == 1), max_batch_bytes=batch_bytes,
+                              shard_index=rank, n_shards=world, allow_regrow=(world == 1 and not disk), max_batch_bytes=batch_bytes,
                               bf_size=bf_size, bf_fp=bf_fp, **engine_kw)
+        self.disk = DiskPieces(self.hc, disk, rank, out_counter_len) if disk else None
         if bc:
             # before the exchange form is chosen: the record exchange declines an engine with a Bloom structure
             self.hc.load_bloom_counter(bc)
@@ -727,6 +734,59 @@ class ShardedCounter(object):
         return self.hc.dump("%s.%d" % (path, self.rank), **kw)
 
 
+class DiskPieces(object):
+    """`count --disk` on one rank: the spill hook of its engine `hc` writes the shard as it stands to piece
+    `<prefix>.<rank>.<i>` (i = 0, 1, ...: `pieces`) with `out_counter_len` bytes a count, and the engine zeroes it and goes
+    on counting.  No rank waits for another: each piece is a database of the GLOBAL geometry that holds only this shard's
+    positions, so merging each rank's pieces and concatenating the results in rank order is the merge of all of them
+    (write_output, concat_shards).  `spill_s`: the seconds spent writing pieces from inside the hook."""
+
+    def __init__(self, hc, prefix, rank, out_counter_len=4):
+        self.hc, self.disk, self.rank, self.out_counter_len = hc, prefix, rank, out_counter_len
+        self.pieces = []
+        self.spill_s = 0.0
+        hc.set_spill(self._spill)
+
+    def _write_piece(self, cmdline=()):
+        """The table as it stands, every record, into the next piece."""
+        path = piece_path(self.disk, self.rank, len(self.pieces))
+        self.pieces.append(path)
+        self.hc.dump(path, out_counter_len=self.out_counter_len, cmdline=cmdline)
+
+    def _spill(self, hc):
+        t0 = time.perf_counter()
+        self._write_piece()
+        self.spill_s += time.perf_counter() - t0
+
+    def discard_pieces(self):
+        """Delete the pieces written so far and number the next one 0 again: the table is about to be cleared and its input
+        counted again (the fall-back of a failed cut check)."""
+        for p in self.pieces:
+            if os.path.exists(p):
+                os.unlink(p)
+        self.pieces = []
+
+    def write_output(self, path, lower=0, upper=UINT64_MAX, cmdline=(), merge=True, unlink=True):
+        """The end of a --disk count on this rank, after done().  A rank that never spilled dumps its shard to `path` with
+        lower / upper, as without --disk.  A rank that spilled writes its table as one more piece; then, with `merge`, it
+        merges its pieces into `path` with lower / upper applied to the sums (merge_pieces) and, with `unlink`, deletes them.
+        merge=False: every piece stays and `path` is not written (nothing is merged; a rank that never spilled then writes
+        its table as its only piece).  Returns the seconds spent merging."""
+        if self.pieces or not merge:
+            self._write_piece(cmdline)
+        if not merge:
+            return 0.0
+        if len(self.pieces) == 0:
+            self.hc.dump(path, lower=lower, upper=upper, out_counter_len=self.out_counter_len, cmdline=cmdline)
+            return 0.0
+        t0 = time.perf_counter()
+        merge_pieces(self.pieces, path, self.hc.header(self.out_counter_len, cmdline), lower, upper)
+        if unlink:
+            for p in self.pieces:
+                os.unlink(p)
+        return time.perf_counter() - t0
+
+
 class BloomBackend(object):
     """What the combination of Bloom counters across ranks needs from the engine; the CUDA engine implements it with kernels.
     A counter is n_words 32-bit words (16 positions each, two bits a position: hit, hit again) whose file body has n_bytes
@@ -870,6 +930,40 @@ def concat_bloom_slices(path, world, header, out=None):
         for r in range(world):
             with open("%s.%d" % (path, r), "rb") as fi:
                 fo.write(fi.read())
+    return out
+
+
+def piece_path(prefix, rank, i):
+    """Piece i of rank `rank` of a --disk count: `<prefix>.<rank>.<i>` (`<prefix>.<rank>` is the rank's shard file)."""
+    return "%s.%d.%d" % (prefix, rank, i)
+
+
+def merge_pieces(pieces, out, header, lower=0, upper=UINT64_MAX):
+    """`jellyfish merge` of the pieces (databases of one geometry) into `out`, -L / -U applied to the sums, by the merge
+    of the command built beside the library (the one `count --disk` ends with); `out` then gets `header` (the count's: the
+    merge itself writes no `canonical` or `val_len`) in front of the merged records."""
+    import shutil
+    import subprocess
+    from . import _lib
+    from .engine import read_header, write_header
+    tool = os.path.join(os.path.dirname(_lib.LIB_PATH), "jellyfish-b200")
+    tmp = out + ".merging"
+    cmd = [tool, "merge", "-o", tmp]
+    if lower:
+        cmd += ["-L", str(lower)]
+    if upper != UINT64_MAX:
+        cmd += ["-U", str(upper)]
+    r = subprocess.run(cmd + list(pieces), stdout=subprocess.PIPE, stderr=subprocess.PIPE)
+    if r.returncode != 0:
+        raise RuntimeError("merging %s failed: %s" % (", ".join(pieces), r.stderr.decode(errors="replace").strip()))
+    try:
+        _, off = read_header(tmp)
+        with open(tmp, "rb") as fi, open(out, "wb") as fo:
+            write_header(fo, header)
+            fi.seek(off)
+            shutil.copyfileobj(fi, fo, 16 << 20)
+    finally:
+        os.unlink(tmp)
     return out
 
 

@@ -95,12 +95,18 @@ class HashCounter(object):
     # -- plumbing ---------------------------------------------------------------------------
     def _check(self, rc):
         if rc:
-            raise JellyfishError(rc, self._lib.jfgpu_last_error(self._h).decode())
+            msg = self._lib.jfgpu_last_error(self._h).decode()
+            cause = getattr(self, "_spill_error", None)
+            if rc == L.ERR_SINK and cause is not None:
+                self._spill_error = None
+                raise JellyfishError(rc, "%s: %s" % (msg, cause)) from cause
+            raise JellyfishError(rc, msg)
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
             self._lib.jfgpu_destroy(self._h)
             self._h = C.c_void_p()
+        self._spill_cb = None
 
     def __del__(self):
         try:
@@ -289,6 +295,23 @@ class HashCounter(object):
         """COUNT (add), PRIME (insert with count 0) or UPDATE (add only to present keys): the two passes
         of `jellyfish count --if` (sub_commands/count_main.cc:288-295)."""
         self._check(self._lib.jfgpu_set_op(self._h, op))
+
+    def set_spill(self, fn):
+        """`count --disk` (include/jfgpu.h: jfgpu_set_spill): when the table is full and may not double (allow_regrow=False,
+        or a shard), fn(self) is called to write it out -- normally self.dump(path, out_counter_len=...) without lower /
+        upper, which dumps the table as it stands -- and the engine then zeroes the table and goes on counting with the same
+        geometry and matrix.  The files it writes are merged at the end (`jellyfish merge`).  An exception raised by fn
+        makes the engine call that filled the table fail with JellyfishError (ERR_SINK).  fn=None removes the hook."""
+        def _hook(ctx, h):
+            try:
+                fn(self)
+                return 0
+            except BaseException as ex:        # (an exception cannot cross the C frames: it is raised by _check)
+                self._spill_error = ex
+                return 1
+        cb = L.SPILL_FN(_hook) if fn is not None else L.SPILL_FN()
+        self._check(self._lib.jfgpu_set_spill(self._h, cb, None))
+        self._spill_cb = cb                     # (the engine calls it for as long as it lives)
 
     def clear(self):
         """Zero the table and statistics (same geometry and hash matrix)."""
